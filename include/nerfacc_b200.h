@@ -28,7 +28,7 @@ extern "C" {
 #define NFA_ERR_ARG (-1)         /* null pointer / negative size / inconsistent sizes */
 #define NFA_ERR_UNSUPPORTED (-2) /* valid request outside what this build implements */
 
-#define NFA_ABI_VERSION 10
+#define NFA_ABI_VERSION 11
 
 typedef void* nfa_stream_t; /* cudaStream_t */
 
@@ -62,7 +62,8 @@ int32_t nfa_intersect_sorted(int32_t n_rays, const float* rays_o, const float* r
 /* Derived cache of OccGridEstimator.binaries (nerfacc/estimators/occ_grid.py:73-76):
  * words  [nfa_occ_words()]        uint64, one per 4x4x4-cell brick,
  * coarse [nfa_occ_coarse_words()] uint32, two bits per brick, 16 bricks per word: bit 0 "some cell set",
- *                                 bit 1 "all 64 cells set" (0 empty, 1 mixed, 3 full),
+ *                                 bit 1 "all 64 cells set" (0 empty, 1 mixed, 3 full); read by
+ *                                 nfa_traverse_generic only,
  * bounds [n_grids * 6]            int32, per level min xyz / max xyz (inclusive, brick units) of the
  *                                 non-empty bricks; min > max when the level is empty. */
 int64_t nfa_occ_words(int32_t n_grids, int32_t rx, int32_t ry, int32_t rz);
@@ -111,15 +112,16 @@ void nfa_debug_set_march_trace(void* buffer);
  *   far_plane for every ray (reference occ_grid.py:154-155 builds those tensors with full_like).  If totals[1] > run_capacity the pool
  *   overflowed: call again with a larger pool (counts and totals are still exact).
  *   t_sorted / t_indices / hits may be NULL when n_grids == 1 (crossings are then
- *   computed in the kernel).  terminate_planes [n_rays] may be NULL.  `bounds` (from nfa_occ_pack,
- *   nullable) lets single-level calls without terminate planes jump over / stop after empty space.
+ *   computed in the kernel).  terminate_planes [n_rays] may be NULL.  `words` and `bounds` come from
+ *   nfa_occ_pack; `bounds` (nullable) lets single-level calls without terminate planes jump over /
+ *   stop after empty space.
  *   workspace: nfa_march_workspace_bytes(n_rays, run_capacity) bytes whose first 64
  *   bytes are zero on first use (the kernels leave it reusable). */
 int64_t nfa_march_workspace_bytes(int32_t n_rays, int64_t run_capacity);
 int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d,
                   const float* near_planes, const float* far_planes, float near_plane, float far_plane,
                   int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
-                  const uint64_t* words, const uint32_t* coarse, const int32_t* bounds, const float* aabbs,
+                  const uint64_t* words, const int32_t* bounds, const float* aabbs,
                   const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,
                   float step_size, int64_t run_capacity, void* workspace, int64_t* totals,
                   int64_t* totals_host, float* terminate_planes, nfa_stream_t stream);

@@ -35,7 +35,7 @@ SIGNATURES = {
     "nfa_debug_set_march_trace": (None, [_c_ptr]),
     "nfa_march_workspace_bytes": (_c_i64, [_c_i32, _c_i64]),
     "nfa_march": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i32, _c_i32, _c_i32, _c_i32,
-                           _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_ptr, _c_ptr,
+                           _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_ptr, _c_ptr,
                            _c_ptr, _c_ptr, _c_ptr]),
     "nfa_expand_samples": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr,
                                     _c_ptr]),
@@ -72,7 +72,7 @@ SIGNATURES = {
     "nfa_pack_info": (_c_i32, [_c_i64, _c_ptr, _c_i32, _c_ptr, _c_ptr, _c_ptr]),
 }
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 _lib = None
 launches = 0  # number of native kernel-launching calls made through this module (bench.py reports it)

@@ -27,35 +27,14 @@
 
 #include "lattice.cuh"
 
-// NFA_BRICK_STEPS == 0 (the shipped setting, see DESIGN.md "march"): the walk never takes whole bricks and the
-// cell loop reads every brick word straight from memory (L1-resident) without consulting the class mip.
-#ifndef NFA_BRICK_STEPS
-#define NFA_BRICK_STEPS 0
-#endif
-// NFA_LOOP_VARIANT: 2 (shipped) = cell loop without branches (selects + one predicated load); 1 = the same loop
-// written with if / else (what the host build of tests/host_sim always uses).  Variant 1 measured slower: each
-// branch region costs a lone warp more than the instructions it skips.
-#ifndef NFA_LOOP_VARIANT
-#define NFA_LOOP_VARIANT 2
-#endif
-#if NFA_BRICK_STEPS
-#define NFA_IF_CLASSES(yes, no) yes
-#else
-#define NFA_IF_CLASSES(yes, no) no
-#endif
-
-// test hook: tests/host_sim counts loop passes (cell steps, brick steps, brick-loop entries); a no-op in the product
-#ifndef NFA_COUNT
-#define NFA_COUNT(i)
-#endif
-
 namespace nfa {
 
 // ---------------------------------------------------------------------------
 // Bit-packed occupancy: 4x4x4-cell bricks, one uint64 per brick, plus a
 // 2-bit-per-brick class mip (bit 0: some cell occupied, bit 1: all 64 cells
-// occupied; so 0 = empty, 1 = mixed, 3 = full).  Derived cache of the estimator's
-// bool `binaries` (reference estimators/occ_grid.py:73-76).
+// occupied; so 0 = empty, 1 = mixed, 3 = full) that the generic traversal reads
+// (march_generic.cuh).  Derived cache of the estimator's bool `binaries`
+// (reference estimators/occ_grid.py:73-76).
 // ---------------------------------------------------------------------------
 struct OccGeom {
     int res[3];   // cells per axis
@@ -76,25 +55,13 @@ NFA_HD OccGeom occ_geom(int n_grids, int rx, int ry, int rz)
 
 struct OccView {
     const uint64_t* words;   // [n_grids * wpl]
-    const uint32_t* coarse;  // class mip, 16 bricks per word: [(n_grids * wpl + 15) / 16]; may live in shared memory
+    const uint32_t* coarse;  // class mip, 16 bricks per word: [(n_grids * wpl + 15) / 16]
     const int32_t* bounds;   // [n_grids][6] bounding box of the non-empty bricks (brick units,
                              // min xyz then max xyz, inclusive; min > max: level empty), or null
     OccGeom g;
 };
 
 enum : uint32_t { kBrickEmpty = 0u, kBrickMixed = 1u, kBrickFull = 3u };
-
-NFA_HD uint32_t occ_class(const uint32_t* mip, int brick)
-{
-    return (mip[brick >> 4] >> ((brick & 15) << 1)) & 3u;
-}
-
-// the 64 cell bits of a brick: only mixed bricks are read from memory
-NFA_HD uint64_t occ_brick_bits(const OccView& occ, int brick)
-{
-    const uint32_t c = occ_class(occ.coarse, brick);
-    return c == kBrickMixed ? occ.words[brick] : (c == kBrickFull ? ~0ull : 0ull);
-}
 
 // ---------------------------------------------------------------------------
 // Ray / box slab test: reference utils_grid.cuh:10-55.
@@ -199,9 +166,6 @@ struct Walk {
     int brick;
     int bit;               // (x&3)<<4 | (y&3)<<2 | (z&3)
     uint64_t word;
-    uint32_t cls;          // class of the current brick (kBrickEmpty / kBrickMixed / kBrickFull)
-    int a_off;             // whole-brick steps are off for the rest of the segment (its end is near)
-    int brick_steps;       // 0: never take whole bricks (measurement aid)
     // state flags (ints, not bools: the compiler would byte-pack bools and shuffle them around)
     int in_seg;
     int open;        // inside a stretch (no EMPTY since it began)
@@ -238,9 +202,6 @@ NFA_HD void walk_init(Walk& w, const float o[3], const float d[3], float near, f
     w.brick = 0;
     w.bit = 0;
     w.word = 0;
-    w.cls = kBrickMixed;
-    w.a_off = 0;
-    w.brick_steps = 1;
     w.in_seg = 0;
     w.open = 0;
     w.joined = 0;
@@ -253,11 +214,7 @@ NFA_HD void walk_init(Walk& w, const float o[3], const float d[3], float near, f
 
 NFA_HD void walk_load_brick(Walk& w, const OccView& occ)
 {
-    NFA_IF_CLASSES(
-        w.cls = occ_class(occ.coarse, w.brick);
-        w.word = w.cls == kBrickMixed ? occ.words[w.brick] : (w.cls == kBrickFull ? ~0ull : 0ull);,
-        w.cls = kBrickMixed;
-        w.word = occ.words[w.brick];)
+    w.word = occ.words[w.brick];
 }
 
 // Steps left on one axis: until the index reaches the overflow index (reference
@@ -349,7 +306,6 @@ NFA_HD void walk_open_segment(Walk& w, const OccView& occ, int level, float lo, 
     w.brick = ((s.cur[0] >> 2) * occ.g.nb[1] + (s.cur[1] >> 2)) * occ.g.nb[2] + (s.cur[2] >> 2) + level * occ.g.wpl;
     w.bit = ((s.cur[0] & 3) << 4) | ((s.cur[1] & 3) << 2) | (s.cur[2] & 3);
     walk_load_brick(w, occ);
-    w.a_off = (NFA_BRICK_STEPS && w.brick_steps) ? 0 : 1;
     w.in_seg = 1;
 }
 
@@ -431,191 +387,81 @@ NFA_HD void walk_run(Walk& w, const Boxes& boxes, const OccView& occ, Buf& buf, 
             walk_open_segment(w, occ, level, lo, hi, boxes.aabb(level));
             continue;
         }
-        // Cells of the current segment, on local scalars.  Two loops take turns (the lanes of a warp follow
-        // unrelated rays; each loop is branch-free inside, and the lanes reconverge between the loops):
-        //   cell loop   one pass = one cell of the reference's loop (grid.cu:184-271), inside mixed bricks;
-        //   brick loop  one pass = one whole 4x4x4 brick whose cells are all empty or all occupied.  Such a brick
-        //               is one EMPTY / OCC event at its exit time, and the exit times are the same f32 chains
-        //               (td (+) dl (+) dl ...) taken four crossings at a time, so the result is bit-identical.
+        // Cells of the current segment, on local scalars: one pass = one cell of the reference's loop
+        // (grid.cu:184-271).  The lanes of a warp follow unrelated rays, so the pass has no branch but the rare
+        // stretch boundary: the axis choice, the counters and the occupancy cursor are selects.
         float tdx = w.tdx, tdy = w.tdy, tdz = w.tdz;
         int remx = w.remx, remy = w.remy, remz = w.remz;
         int bit = w.bit, brick = w.brick;
         uint64_t word = w.word;
-        uint32_t cls = w.cls;
-        int open = w.open, joined = w.joined, a_off = w.a_off;
+        int open = w.open, joined = w.joined;
         float pend = w.pend, d_open = w.d_open;
         const float dlx = w.dlx, dly = w.dly, dlz = w.dlz, seg_hi = w.seg_hi, t_stop = w.t_stop;
         const int dbx = w.dbx, dby = w.dby, dbz = w.dbz, sbx = w.sbx, sby = w.sby, sbz = w.sbz;
         int in_seg = 1;
         while (in_seg && n_desc < cap) {
-            // ---------------- cell loop: while the brick is mixed (or brick steps are off)
-            while (in_seg && n_desc < cap && (cls == kBrickMixed || a_off)) {
-                NFA_COUNT(0);
-                const float tt = f_min(f_min(tdx, f_min(tdy, tdz)), seg_hi);  // grid.cu:185-186
-                // --- the DDA step first (utils_grid.cuh:116-142: x only if strictly smallest, else y if strictly
-                // below z, else z).  It does not depend on the occupancy, and the brick word that the previous pass
-                // may have requested has these ~30 instructions to arrive before the bit test below reads it.
-                // The occupancy cursor moves along the stepped axis: add inside the axis' 2-bit field of `bit`; a
-                // carry / borrow out of the field means the step left the brick.
-                const bool mx = tdx < tdy && tdx < tdz;
-                const bool my = !mx && (tdy < tdz);
-#if NFA_LOOP_VARIANT >= 2
-                const bool mz = !mx && !my;
-                tdx = mx ? f_add(tdx, dlx) : tdx;
-                tdy = my ? f_add(tdy, dly) : tdy;
-                tdz = mz ? f_add(tdz, dlz) : tdz;
-                remx -= mx ? 1 : 0;
-                remy -= my ? 1 : 0;
-                remz -= mz ? 1 : 0;
-                const int db = mx ? dbx : (my ? dby : dbz);
-                const int mk = mx ? 0x30 : (my ? 0x0c : 0x03);
-                const int sb = mx ? sbx : (my ? sby : sbz);
+            const float tt = f_min(f_min(tdx, f_min(tdy, tdz)), seg_hi);  // grid.cu:185-186
+            // --- the DDA step first (utils_grid.cuh:116-142: x only if strictly smallest, else y if strictly
+            // below z, else z).  It does not depend on the occupancy, and the brick word that the previous pass
+            // may have requested has these ~30 instructions to arrive before the bit test below reads it.
+            // The occupancy cursor moves along the stepped axis: add inside the axis' 2-bit field of `bit`; a
+            // carry / borrow out of the field means the step left the brick.
+            const bool mx = tdx < tdy && tdx < tdz;
+            const bool my = !mx && (tdy < tdz);
+            const bool mz = !mx && !my;
+            tdx = mx ? f_add(tdx, dlx) : tdx;
+            tdy = my ? f_add(tdy, dly) : tdy;
+            tdz = mz ? f_add(tdz, dlz) : tdz;
+            remx -= mx ? 1 : 0;
+            remy -= my ? 1 : 0;
+            remz -= mz ? 1 : 0;
+            const int db = mx ? dbx : (my ? dby : dbz);
+            const int mk = mx ? 0x30 : (my ? 0x0c : 0x03);
+            const int sb = mx ? sbx : (my ? sby : sbz);
+            const int nb = bit + db;
+            const bool crossed = ((nb ^ bit) & ~mk) != 0;
+            const int bit_next = (bit & ~mk) | (nb & mk);
+            // only the stepped counter changed and all three were positive: one of them is 0 <=> that one is
+            const int rem_min = remx < remy ? (remx < remz ? remx : remz) : (remy < remz ? remy : remz);
+            const bool stop = rem_min == 0 || tt >= t_stop;  // overflow index / grid edge, or past the occupied box
+
+            // --- the cell just left: OCC(tt) / EMPTY(tt)
+            const int occd = (int)((uint32_t)(word >> bit) & 1u);
+            if (occd != open) {  // a stretch opens (its pend is frozen from here on) or closes
+                if (open) {      // EMPTY(tt) closes the stretch
+                    buf.put(n_desc++, pend, d_open, joined != 0);
+                    pend = -INFINITY;
+                } else {
+                    joined = 0;
+                }
+                open = occd;
+            }
+            if (occd) d_open = tt;             // the stretch grows
+            else pend = f_max(pend, tt);       // the skip target moves on
+
+            // --- commit the step
+            bit = bit_next;
+#ifdef __CUDA_ARCH__
+            in_seg = stop ? 0 : 1;
+            brick += crossed ? sb : 0;
+            {   // predicated load: a branch here costs more than the load it skips
+                const uint64_t* src = occ.words + brick;
+                asm volatile("{\n.reg .pred p;\nsetp.ne.s32 p, %2, 0;\n@p ld.global.nc.u64 %0, [%1];\n}"
+                             : "+l"(word) : "l"(src), "r"((int)(crossed && !stop)));
+            }
 #else
-                int db, mk, sb;
-                if (mx) { tdx = f_add(tdx, dlx); --remx; db = dbx; mk = 0x30; sb = sbx; }
-                else if (my) { tdy = f_add(tdy, dly); --remy; db = dby; mk = 0x0c; sb = sby; }
-                else { tdz = f_add(tdz, dlz); --remz; db = dbz; mk = 0x03; sb = sbz; }
+            if (stop) {
+                in_seg = 0;
+            } else if (crossed) {
+                brick += sb;
+                word = occ.words[brick];
+            }
 #endif
-                const int nb = bit + db;
-                const bool crossed = ((nb ^ bit) & ~mk) != 0;
-                const int bit_next = (bit & ~mk) | (nb & mk);
-                // only the stepped counter changed and all three were positive: one of them is 0 <=> that one is
-                const int rem_min = remx < remy ? (remx < remz ? remx : remz) : (remy < remz ? remy : remz);
-                const bool stop = rem_min == 0 || tt >= t_stop;  // overflow index / grid edge, or past the occupied box
-
-                // --- the cell just left: OCC(tt) / EMPTY(tt)
-                const int occd = (int)((uint32_t)(word >> bit) & 1u);
-                if (occd != open) {  // a stretch opens (its pend is frozen from here on) or closes
-                    if (open) {      // EMPTY(tt) closes the stretch
-                        buf.put(n_desc++, pend, d_open, joined != 0);
-                        pend = -INFINITY;
-                    } else {
-                        joined = 0;
-                    }
-                    open = occd;
-                }
-                if (occd) d_open = tt;             // the stretch grows
-                else pend = f_max(pend, tt);       // the skip target moves on
-
-                // --- commit the step
-                bit = bit_next;
-#if NFA_LOOP_VARIANT >= 2 && !NFA_BRICK_STEPS && defined(__CUDA_ARCH__)
-                in_seg = stop ? 0 : 1;
-                brick += crossed ? sb : 0;
-                {   // predicated load: a branch here costs more than the load it skips
-                    const uint64_t* src = occ.words + brick;
-                    asm volatile("{\n.reg .pred p;\nsetp.ne.s32 p, %2, 0;\n@p ld.global.nc.u64 %0, [%1];\n}"
-                                 : "+l"(word) : "l"(src), "r"((int)(crossed && !stop)));
-                }
-#else
-                if (stop) {
-                    in_seg = 0;
-                } else if (crossed) {
-                    brick += sb;
-                    NFA_IF_CLASSES(
-                        if (a_off) {  // no brick steps for this ray any more: the class is of no use
-                            word = occ.words[brick];
-                        } else {
-                            cls = occ_class(occ.coarse, brick);
-                            word = cls == kBrickMixed ? occ.words[brick] : (cls == kBrickFull ? ~0ull : 0ull);
-                        },
-                        word = occ.words[brick];)
-                }
-#endif
-            }
-            if (!NFA_BRICK_STEPS || !in_seg || n_desc >= cap) break;
-
-            // ---------------- brick loop.  Per axis: q = crossings left inside the brick, B = time of the crossing
-            // that leaves it (q more chain adds), cnt = bricks that may still be taken whole along this axis
-            // before the one in which the walk ends (its end is a cell-level event: the cell loop finds it).
-            // While bricks are taken whole only the axis that is crossed is kept up to date; (td, rem, bit field)
-            // of the other two are a snapshot of the moment they last were, and are brought forward when the cell
-            // loop takes over again (the crossings that precede the entry (E_in, axis a_in) of the current brick).
-            int qx, qy, qz, cntx, cnty, cntz;
-            float Bx, By, Bz;
-            {
-                const int fx = (bit >> 4) & 3, fy = (bit >> 2) & 3, fz = bit & 3;
-                const int still = 0x3fffffff;
-                qx = dbx > 0 ? 3 - fx : (dbx < 0 ? fx : still);
-                qy = dby > 0 ? 3 - fy : (dby < 0 ? fy : still);
-                qz = dbz > 0 ? 3 - fz : (dbz < 0 ? fz : still);
-                const float x1 = f_add(tdx, dlx), x2 = f_add(x1, dlx), x3 = f_add(x2, dlx);
-                const float y1 = f_add(tdy, dly), y2 = f_add(y1, dly), y3 = f_add(y2, dly);
-                const float z1 = f_add(tdz, dlz), z2 = f_add(z1, dlz), z3 = f_add(z2, dlz);
-                Bx = qx == 0 ? tdx : (qx == 1 ? x1 : (qx == 2 ? x2 : (qx == 3 ? x3 : INFINITY)));
-                By = qy == 0 ? tdy : (qy == 1 ? y1 : (qy == 2 ? y2 : (qy == 3 ? y3 : INFINITY)));
-                Bz = qz == 0 ? tdz : (qz == 1 ? z1 : (qz == 2 ? z2 : (qz == 3 ? z3 : INFINITY)));
-                cntx = remx > qx + 1 ? (remx - qx + 2) >> 2 : 0;
-                cnty = remy > qy + 1 ? (remy - qy + 2) >> 2 : 0;
-                cntz = remz > qz + 1 ? (remz - qz + 2) >> 2 : 0;
-            }
-            NFA_COUNT(2);
-            float E_in = -INFINITY;
-            int a_in = 0;
-            if (cntx == 0 || cnty == 0 || cntz == 0) a_off = 1;  // the walk ends in this brick: cells only from here
-            while (in_seg && n_desc < cap && cls != kBrickMixed && !a_off) {
-                NFA_COUNT(1);
-                const bool mx = Bx < By && Bx < Bz;
-                const bool my = !mx && (By < Bz);
-                const bool mz = !mx && !my;
-                const float E = mx ? Bx : (my ? By : Bz);
-                const float tt = f_min(E, seg_hi);
-                const int occd = cls == kBrickFull ? 1 : 0;
-                if (occd != open) {
-                    if (open) {
-                        buf.put(n_desc++, pend, d_open, joined != 0);
-                        pend = -INFINITY;
-                    } else {
-                        joined = 0;
-                    }
-                    open = occd;
-                }
-                d_open = occd ? tt : d_open;
-                pend = occd ? pend : f_max(pend, tt);
-                if (tt >= t_stop) {
-                    in_seg = 0;
-                    break;
-                }
-                // cross into the next brick along the chosen axis: that axis is up to date again
-                const float n0 = f_add(E, mx ? dlx : (my ? dly : dlz));
-                const float n1 = f_add(n0, mx ? dlx : (my ? dly : dlz));
-                const float n2 = f_add(n1, mx ? dlx : (my ? dly : dlz));
-                const float n3 = f_add(n2, mx ? dlx : (my ? dly : dlz));
-                if (mx) { remx -= qx + 1; qx = 3; tdx = n0; Bx = n3; cntx -= 1; bit = (bit & ~0x30) | (dbx > 0 ? 0 : 0x30); }
-                if (my) { remy -= qy + 1; qy = 3; tdy = n0; By = n3; cnty -= 1; bit = (bit & ~0x0c) | (dby > 0 ? 0 : 0x0c); }
-                if (mz) { remz -= qz + 1; qz = 3; tdz = n0; Bz = n3; cntz -= 1; bit = (bit & ~0x03) | (dbz > 0 ? 0 : 0x03); }
-                brick += mx ? sbx : (my ? sby : sbz);
-                cls = occ_class(occ.coarse, brick);
-                E_in = E;
-                a_in = mx ? 0 : (my ? 1 : 2);
-                if ((mx ? cntx : (my ? cnty : cntz)) == 0) a_off = 1;
-            }
-            // hand back to the cell loop: bring the two snapshot axes forward to (E_in, a_in).  An event of axis b
-            // at time c precedes it when c < E_in, or c == E_in and b wins the DDA's tie (z before y before x).
-            {
-                const float x1 = f_add(tdx, dlx), x2 = f_add(x1, dlx);
-                const float y1 = f_add(tdy, dly), y2 = f_add(y1, dly);
-                const float z1 = f_add(tdz, dlz), z2 = f_add(z1, dlz);
-                const bool xw = false, yw = a_in < 1, zw = a_in < 2;  // does the axis win a tie against a_in
-                const int mxn = a_in == 0 ? 0 : ((tdx < E_in || (xw && tdx == E_in)) + (x1 < E_in || (xw && x1 == E_in)) +
-                                                 (x2 < E_in || (xw && x2 == E_in)));
-                const int myn = a_in == 1 ? 0 : ((tdy < E_in || (yw && tdy == E_in)) + (y1 < E_in || (yw && y1 == E_in)) +
-                                                 (y2 < E_in || (yw && y2 == E_in)));
-                const int mzn = a_in == 2 ? 0 : ((tdz < E_in || (zw && tdz == E_in)) + (z1 < E_in || (zw && z1 == E_in)) +
-                                                 (z2 < E_in || (zw && z2 == E_in)));
-                const float x3 = f_add(x2, dlx), y3 = f_add(y2, dly), z3 = f_add(z2, dlz);
-                tdx = mxn == 0 ? tdx : (mxn == 1 ? x1 : (mxn == 2 ? x2 : x3));
-                tdy = myn == 0 ? tdy : (myn == 1 ? y1 : (myn == 2 ? y2 : y3));
-                tdz = mzn == 0 ? tdz : (mzn == 1 ? z1 : (mzn == 2 ? z2 : z3));
-                remx -= mxn; remy -= myn; remz -= mzn;
-                bit += dbx * mxn + dby * myn + dbz * mzn;
-                word = cls == kBrickMixed ? occ.words[brick] : (cls == kBrickFull ? ~0ull : 0ull);
-            }
         }
         w.tdx = tdx; w.tdy = tdy; w.tdz = tdz;
         w.remx = remx; w.remy = remy; w.remz = remz;
-        w.bit = bit; w.brick = brick; w.word = word; w.cls = cls;
-        w.open = open; w.joined = joined; w.a_off = a_off;
+        w.bit = bit; w.brick = brick; w.word = word;
+        w.open = open; w.joined = joined;
         w.pend = pend; w.d_open = d_open;
         w.in_seg = in_seg;
     }

@@ -13,6 +13,18 @@
 
 namespace nfa {
 
+NFA_HD uint32_t occ_class(const uint32_t* mip, int brick)
+{
+    return (mip[brick >> 4] >> ((brick & 15) << 1)) & 3u;
+}
+
+// the 64 cell bits of a brick: only mixed bricks are read from memory
+NFA_HD uint64_t occ_brick_bits(const OccView& occ, int brick)
+{
+    const uint32_t c = occ_class(occ.coarse, brick);
+    return c == kBrickMixed ? occ.words[brick] : (c == kBrickFull ? ~0ull : 0ull);
+}
+
 NFA_HD bool occ_test(const OccView& v, int level, int ix, int iy, int iz)
 {
     const int b = ((ix >> 2) * v.g.nb[1] + (iy >> 2)) * v.g.nb[2] + (iz >> 2) + level * v.g.wpl;

@@ -5,7 +5,7 @@
 // nerfacc/cuda/csrc/grid.cu:320-474):
 //
 //   occ_pack_kernel   bool grid -> 4x4x4 brick words + 2-bit/brick class mip (cached per grid version)
-//   march_kernel      1 thread / ray, 128 rays / CTA.  Ray tile and brick mip staged
+//   march_kernel      1 thread / ray, march_tile_rays() rays / CTA.  Ray tile staged
 //                     into shared memory with cp.async.bulk (TMA 1-D) + mbarrier; the
 //                     tile's rays are ordered by expected walk length so that the lanes
 //                     of a warp finish together.  Phase 1: pure DDA walk recording
@@ -28,7 +28,6 @@
 // f32 chains (march) and by HBM stores (expand).  See DESIGN.md.
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "../../include/nerfacc_b200.h"
 #include "sm_count.cuh"
@@ -40,9 +39,6 @@
 namespace nfa {
 
 constexpr int kMaxTileRays = 512;   // rays per CTA in the march / offsets kernels: march_tile_rays(), <= this
-#ifndef NFA_POOL_ONE_ATOMIC
-#define NFA_POOL_ONE_ATOMIC 1
-#endif
 constexpr int kDescSlots = 8;       // stretch descriptors buffered per ray between the two march phases ...
 constexpr int kDescSlotsWide = 16;  // ... and when one wave holds every ray (shared memory to spare): no second round
 constexpr int kSortBuckets = 256;   // counting sort of a tile's rays by expected walk length
@@ -54,12 +50,6 @@ constexpr int kSortBuckets = 256;   // counting sort of a tile's rays by expecte
 // (several waves) use 256.
 inline int march_tile_rays(int32_t n_rays)
 {
-    static const int forced = [] {  // measurement aid: NFA_MARCH_TILE=<multiple of 32> pins the tile size
-        const char* e = getenv("NFA_MARCH_TILE");
-        const int v = e ? atoi(e) : 0;
-        return (v >= 32 && v <= kMaxTileRays && v % 32 == 0) ? v : 0;
-    }();
-    if (forced) return forced;
     const int kSMs = kNumSMs;
     if (n_rays <= 32) return 32;
     if ((int64_t)n_rays > (int64_t)kSMs * 2048) return 256;
@@ -244,8 +234,6 @@ struct MarchParams {
     float near_plane, far_plane;
     OccGeom g;
     const uint64_t* words;
-    const uint32_t* coarse;
-    int32_t coarse_words;  // padded count (multiple of 4)
     const int32_t* bounds;  // occupied-brick bounding boxes (nullable)
     const float* aabbs;
     const float* t_sorted;
@@ -253,7 +241,6 @@ struct MarchParams {
     const uint8_t* hits;
     float step_size;
     LatTable lat_table;   // lattice points at the binade starts, from the uniform near plane (n = 0: none)
-    int32_t brick_steps;  // warps per tile (the longest rays) that may take whole bricks; needs -DNFA_BRICK_STEPS=1
     unsigned long long* trace;  // measurement aid (nfa_debug_set_march_trace): 8 x u64 per warp, or null
     Workspace ws;
     int64_t* totals;
@@ -295,13 +282,13 @@ __device__ __forceinline__ void emit_runs(const RunOut& out, uint32_t ray, uint3
 }
 
 // dynamic shared memory of the march kernel (tile = blockDim.x rays):
-//   [class mip (kSmemCoarse)] [o: 3 tile f32] [d: 3 tile f32] [pend: slots tile] [open: slots tile] [order: tile u32]
-__host__ __device__ inline size_t march_smem_bytes(int tile, size_t coarse_bytes, int slots)
+//   [o: 3 tile f32] [d: 3 tile f32] [pend: slots tile] [open: slots tile] [order: tile u32]
+__host__ __device__ inline size_t march_smem_bytes(int tile, int slots)
 {
-    return coarse_bytes + (size_t)tile * 4 * (3 + 3 + 2 * slots + 1);
+    return (size_t)tile * 4 * (3 + 3 + 2 * slots + 1);
 }
 
-template <bool kSingle, bool kSmemCoarse, int kSlots>
+template <bool kSingle, int kSlots>
 __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p)
 {
     extern __shared__ __align__(16) uint32_t s_dyn[];
@@ -322,8 +309,7 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
     const int tile = blockIdx.x;
     const int r0 = tile * T;
     const int nr = min(T, p.n_rays - r0);
-    uint32_t* s_coarse = s_dyn;
-    float* s_o = reinterpret_cast<float*>(s_dyn + (kSmemCoarse ? p.coarse_words : 0));
+    float* s_o = reinterpret_cast<float*>(s_dyn);
     float* s_d = s_o + 3 * T;
     float* s_pend = s_d + 3 * T;
     constexpr int S = kSlots;  // stretch descriptors buffered per ray
@@ -332,12 +318,11 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
     float* s_tail = reinterpret_cast<float*>(s_sort);  // lattice point after a ray's last stretch: each thread has read
                                                        // its s_sort slot long before a lane of its warp writes here
 
-    // ---- stage the ray tile (and the class mip) into shared memory: TMA bulk copies + mbarrier
+    // ---- stage the ray tile into shared memory: TMA bulk copies + mbarrier
     const float* g_o = p.rays_o + (int64_t)r0 * 3;
     const float* g_d = p.rays_d + (int64_t)r0 * 3;
     const uint32_t ray_bytes = (uint32_t)nr * 12u;
     const bool bulk_rays = ((ray_bytes & 15u) == 0u) && ((((uintptr_t)g_o) | ((uintptr_t)g_d)) & 15u) == 0u;
-    const bool bulk_coarse = kSmemCoarse && ((((uintptr_t)p.coarse) & 15u) == 0u);
     if (tid == 0) mbar_init(&s_bar, 1);
     if (kSingle && tid < kSortBuckets) s_hist[tid] = 0u;
     if (kSingle && T < kSortBuckets) {
@@ -345,24 +330,17 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
     }
     __syncthreads();
     if (tid == 0) {
-        uint32_t bytes = 0;
-        if (bulk_rays) bytes += 2u * ray_bytes;
-        if (bulk_coarse) bytes += (uint32_t)p.coarse_words * 4u;
-        mbar_expect_tx(&s_bar, bytes);
+        mbar_expect_tx(&s_bar, bulk_rays ? 2u * ray_bytes : 0u);
         if (bulk_rays) {
             bulk_g2s(s_o, g_o, ray_bytes, &s_bar);
             bulk_g2s(s_d, g_d, ray_bytes, &s_bar);
         }
-        if (bulk_coarse) bulk_g2s(s_coarse, p.coarse, (uint32_t)p.coarse_words * 4u, &s_bar);
     }
     if (!bulk_rays) {
         for (int i = tid; i < nr * 3; i += T) {
             s_o[i] = g_o[i];
             s_d[i] = g_d[i];
         }
-    }
-    if (kSmemCoarse && !bulk_coarse) {
-        for (int i = tid; i < p.coarse_words; i += T) s_coarse[i] = p.coarse[i];
     }
     mbar_wait(&s_bar, 0);
     __syncthreads();
@@ -439,7 +417,7 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
     // ---- two-phase march (march.cuh) ---------------------------------------
     OccView occ;
     occ.words = p.words;
-    occ.coarse = kSmemCoarse ? s_coarse : p.coarse;
+    occ.coarse = nullptr;  // the march reads brick words only
     occ.bounds = p.bounds;
     occ.g = p.g;
     const Lattice L = lat_make(p.step_size);
@@ -452,9 +430,6 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
     w.done = active ? 0 : 1;
     // nothing after the last occupied cell is observable without a terminate plane on one level
     w.accel = (kSingle && p.terminate == nullptr) ? 1 : 0;
-    // whole-brick steps (when compiled in) only for the tile's longest rays: after the sort these sit in the last
-    // warps, pass near the middle of the occupied region and so cross the same kinds of brick together
-    w.brick_steps = (p.brick_steps > 0 && tid >= T - 32 * p.brick_steps) ? 1 : 0;
     SmemBuf buf;
     buf.pend = s_pend;
     buf.open = s_open;
@@ -521,7 +496,6 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
                 }
             }
             __syncwarp();
-#if NFA_POOL_ONE_ATOMIC
             // back to one lane per ray: count the ray's runs (stretches that hold a sample), take the pool slots of the
             // whole warp with ONE atomic (its round trip to L2 per stretch index was a fifth of this phase), then
             // add up the offsets and write the records -- plain per-lane loops, no warp-wide step inside
@@ -563,14 +537,6 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
                     lat_take(m, s_pend[j * T + tid], __float_as_uint(s_open[j * T + tid]), out);
                 }
             }
-#else
-            for (int j = 0; j < maxd; ++j) {
-                RunOut out;
-                out.valid = false;
-                if (j < n_desc) lat_take(m, s_pend[j * T + tid], __float_as_uint(s_open[j * T + tid]), out);
-                emit_runs(out, (uint32_t)r, (uint32_t)tile, p.ws, lane);
-            }
-#endif
             if (n_desc > 0 && m.ok) m.t = s_tail[tid];
         } else {
             for (int j = 0; j < maxd; ++j) {
@@ -1117,6 +1083,22 @@ static inline int32_t launch_status()
 
 static unsigned long long* g_march_trace = nullptr;
 
+// One march launch; the dynamic shared memory limit is raised above the 48 KiB default once per instantiation and
+// device.
+template <bool kSingle, int kSlots>
+static void launch_march(const MarchParams& p, int tiles, int threads, cudaStream_t s)
+{
+    const size_t dyn = march_smem_bytes(threads, kSlots);
+    static bool raised[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dyn > 40 * 1024 && !raised[dev & 63]) {
+        cudaFuncSetAttribute(march_kernel<kSingle, kSlots>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        raised[dev & 63] = true;
+    }
+    march_kernel<kSingle, kSlots><<<tiles, threads, dyn, s>>>(p);
+}
+
 extern "C" {
 
 // measurement aid, not part of the product path: per-warp time stamps of the next nfa_march launches go to
@@ -1196,7 +1178,7 @@ int64_t nfa_march_workspace_bytes(int32_t n_rays, int64_t run_capacity)
 int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
                   const float* far_planes, float near_plane, float far_plane, int32_t n_grids, int32_t rx,
                   int32_t ry, int32_t rz,
-                  const uint64_t* words, const uint32_t* coarse, const int32_t* bounds, const float* aabbs,
+                  const uint64_t* words, const int32_t* bounds, const float* aabbs,
                   const float* t_sorted, const int64_t* t_indices, const uint8_t* hits, float step_size,
                   int64_t run_capacity, void* workspace, int64_t* totals, int64_t* totals_host,
                   float* terminate_planes, nfa_stream_t stream)
@@ -1211,7 +1193,7 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
         if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
         return (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
     }
-    if (!rays_o || !rays_d || !words || !coarse || !aabbs || !workspace)
+    if (!rays_o || !rays_d || !words || !aabbs || !workspace)
         return NFA_ERR_ARG;
     const bool have_sorted = t_sorted && t_indices && hits;
     if (!have_sorted && n_grids != 1) return NFA_ERR_ARG;
@@ -1225,19 +1207,12 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
     p.far_plane = far_plane;
     p.g = occ_geom(n_grids, rx, ry, rz);
     p.words = words;
-    p.coarse = coarse;
-    p.coarse_words = (int32_t)occ_coarse_words(p.g);
     p.bounds = bounds;
     p.aabbs = aabbs;
     p.t_sorted = have_sorted ? t_sorted : nullptr;
     p.t_indices = have_sorted ? t_indices : nullptr;
     p.hits = have_sorted ? hits : nullptr;
     p.step_size = step_size;
-    static const int brick_steps = [] {  // number of (longest-ray) warps per tile that take whole bricks
-        const char* e = getenv("NFA_MARCH_BRICK_WARPS");
-        return e ? atoi(e) : 2;
-    }();
-    p.brick_steps = brick_steps;
     p.trace = g_march_trace;
     p.lat_table.n = 0;
     p.lat_table.e0 = 0;
@@ -1257,41 +1232,16 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
     p.totals = totals;
     p.totals_host = totals_host;
     p.terminate = terminate_planes;
-    const int tiles = p.ws.n_tiles, tile_rays = p.ws.tile_rays;
-    const int threads = tile_rays;
-    const size_t coarse_bytes = (size_t)p.coarse_words * 4;
-    // keep the class mip in shared memory while it leaves room for the tile's own buffers (256^3: 64 KiB)
-    const bool smem_coarse = NFA_BRICK_STEPS && coarse_bytes <= 128 * 1024;  // only the brick loop reads the mip
+    const int tiles = p.ws.n_tiles, threads = p.ws.tile_rays;
     // one wave (every tile resident at once, at most two per SM): room for twice the descriptor slots
-    static const int slots_cfg = [] {  // measurement aid: NFA_MARCH_SLOTS=8|16 pins it
-        const char* e = getenv("NFA_MARCH_SLOTS");
-        return e ? atoi(e) : 0;
-    }();
-    const bool wide = slots_cfg ? slots_cfg == kDescSlotsWide : (tiles <= 2 * kNumSMs && threads >= 224);
-    const size_t dyn = march_smem_bytes(threads, smem_coarse ? coarse_bytes : 0, wide ? kDescSlotsWide : kDescSlots);
-#define NFA_LAUNCH_MARCH(S, C, W)                                                                       \
-    do {                                                                                                \
-        static bool raised[64] = {}; /* once per instantiation and device: above the 48 KiB default */  \
-        int dev_ = 0;                                                                                   \
-        cudaGetDevice(&dev_);                                                                           \
-        if (dyn > 40 * 1024 && !raised[dev_ & 63]) {                                                    \
-            cudaFuncSetAttribute(march_kernel<S, C, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
-            raised[dev_ & 63] = true;                                                                   \
-        }                                                                                               \
-        march_kernel<S, C, W><<<tiles, threads, dyn, s>>>(p);                                           \
-    } while (0)
-#define NFA_LAUNCH_MARCH_SC(S, C)                                                  \
-    do {                                                                           \
-        if (wide) NFA_LAUNCH_MARCH(S, C, kDescSlotsWide);                          \
-        else NFA_LAUNCH_MARCH(S, C, kDescSlots);                                   \
-    } while (0)
+    const bool wide = tiles <= 2 * kNumSMs && threads >= 224;
     if (!have_sorted) {
-        if (smem_coarse) NFA_LAUNCH_MARCH_SC(true, NFA_BRICK_STEPS != 0); else NFA_LAUNCH_MARCH_SC(true, false);
+        if (wide) launch_march<true, kDescSlotsWide>(p, tiles, threads, s);
+        else launch_march<true, kDescSlots>(p, tiles, threads, s);
     } else {
-        if (smem_coarse) NFA_LAUNCH_MARCH_SC(false, NFA_BRICK_STEPS != 0); else NFA_LAUNCH_MARCH_SC(false, false);
+        if (wide) launch_march<false, kDescSlotsWide>(p, tiles, threads, s);
+        else launch_march<false, kDescSlots>(p, tiles, threads, s);
     }
-#undef NFA_LAUNCH_MARCH_SC
-#undef NFA_LAUNCH_MARCH
     return launch_status();
 }
 

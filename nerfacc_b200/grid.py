@@ -216,7 +216,7 @@ class _MarchJob:
         sc, occ = self.sc, self.occ
         _lib.call("nfa_march", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(near_planes),
                   _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz, _lib.ptr(occ.words),
-                  _lib.ptr(occ.coarse), _lib.ptr(occ.bounds), _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices),
+                  _lib.ptr(occ.bounds), _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices),
                   _lib.ptr(hits), self.step_size, sc.run_capacity, _lib.ptr(sc.workspace), _lib.ptr(sc.totals_dev),
                   _lib.ptr(sc.totals_host), _lib.ptr(self.term))
         # on the stream (of THIS device) the march was launched on: the default `record()` would use the current

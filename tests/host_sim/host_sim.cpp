@@ -10,11 +10,6 @@
 #include <cstring>
 #include <vector>
 
-#include <vector>
-static long g_walk_counts[3];
-static std::vector<unsigned char> g_trace;   // per-ray event log of the walk (0 cell step, 1 brick step, 2 brick-loop entry, 255 end of ray)
-static bool g_trace_on = false;
-#define NFA_COUNT(i) (++g_walk_counts[i], g_trace_on ? g_trace.push_back((unsigned char)(i)) : (void)0)
 #include "../../nerfacc_b200/csrc/occ_pack.cuh"
 #include "../../nerfacc_b200/csrc/expand.cuh"
 #include "../../nerfacc_b200/csrc/march_generic.cuh"
@@ -23,17 +18,6 @@ static bool g_trace_on = false;
 using namespace nfa;
 
 extern "C" {
-
-// loop passes of the walk since the last reset: cell steps, whole-brick steps, brick-loop entries
-void sim_walk_counts(long* out, int reset)
-{
-    for (int i = 0; i < 3; ++i) { out[i] = g_walk_counts[i]; if (reset) g_walk_counts[i] = 0; }
-}
-
-// event log of the walk: sim_trace(1) clears and starts logging; sim_trace_read copies it out
-void sim_trace(int on) { g_trace_on = on != 0; g_trace.clear(); }
-long sim_trace_size(void) { return (long)g_trace.size(); }
-void sim_trace_read(unsigned char* out) { memcpy(out, g_trace.data(), g_trace.size()); }
 
 // serial reference chain: k steps of t += dt
 float sim_chain(float t, float dt, uint32_t k)
@@ -253,7 +237,6 @@ int64_t sim_march(int32_t n_rays, const float* rays_o, const float* rays_d,
                           hits + (int64_t)r * n_grids};
             term = march_one(b, occ, rays_o + 3 * r, rays_d + 3 * r, near_planes[r], far_planes[r], L, m, vt, vn, 0);
         }
-        if (g_trace_on) g_trace.push_back(255);
         n_samples[r] = m.n_samples;
         n_runs[r] = m.n_runs;
         terminate[r] = term;

@@ -104,15 +104,16 @@ void sim_occ_pack(int n_grids, int rx, int ry, int rz, const uint8_t* binaries, 
 
 static long g_by_stretch_rounds, g_tables;
 
-// descriptor buffer with the same capacity as the device kernel's per-ray slots
+// descriptor buffer with the capacity of the device kernel's per-ray slots (march_kernel: 8, or 16 when wide)
+template <int kSlots>
 struct HostBuf {
-    enum { K = 8 };
+    enum { K = kSlots };
     float pend[K], open[K];
     bool joined[K];
     void put(int j, float p, float o, bool jn) { pend[j] = p; open[j] = o; joined[j] = jn; }
 };
 
-template <class Boxes>
+template <int kSlots, class Boxes>
 static float march_one(const Boxes& boxes, const OccView& occ, const float* o, const float* d, float near, float far,
                        const Lattice& L, LatState& m, std::vector<float>& vt, std::vector<uint32_t>& vn, int accel)
 {
@@ -120,12 +121,12 @@ static float march_one(const Boxes& boxes, const OccView& occ, const float* o, c
     walk_init(w, o, d, near, far);
     w.accel = accel;
     lat_init(m, L, near);
-    HostBuf buf;
+    HostBuf<kSlots> buf;
     int n_desc = 0;
     RunOut out;
     // same chunked structure as the kernel: walk until the buffer is full, then flush it
     for (long guard = 0; guard < (1L << 26); ++guard) {
-        walk_run(w, boxes, occ, buf, n_desc, HostBuf::K);
+        walk_run(w, boxes, occ, buf, n_desc, kSlots);
         for (int j = 0; j < n_desc; ++j) {
             lat_consume(m, buf.pend[j], buf.open[j], buf.joined[j], out);
             if (out.valid) { vt.push_back(out.t_first); vn.push_back(out.n); }
@@ -140,6 +141,7 @@ static float march_one(const Boxes& boxes, const OccView& occ, const float* o, c
 
 // The kernel's phase 2 for one grid level: a round's stretches handled independently from one anchor
 // (march.cuh: lat_anchor / lat_stretch / lat_take), the way march_kernel deals them out to the lanes of a warp.
+template <int kSlots>
 static float march_one_by_stretch(const OccView& occ, const float* box, const float* o, const float* d, float near,
                                   float far, const Lattice& L, LatState& m, std::vector<float>& vt,
                                   std::vector<uint32_t>& vn)
@@ -152,11 +154,11 @@ static float march_one_by_stretch(const OccView& occ, const float* box, const fl
     LatTable table;  // (the kernel gets it from the host, for a uniform near plane; here every ray builds its own)
     lat_table_build(L, near, table);
     if (table.n > 0) ++g_tables;
-    HostBuf buf;
+    HostBuf<kSlots> buf;
     int n_desc = 0;
     RunOut out;
     for (long guard = 0; guard < (1L << 26); ++guard) {
-        walk_run(w, boxes, occ, buf, n_desc, HostBuf::K);
+        walk_run(w, boxes, occ, buf, n_desc, kSlots);
         bool any_joined = false;
         for (int j = 0; j < n_desc; ++j) any_joined = any_joined || buf.joined[j];
         if (any_joined) {
@@ -173,8 +175,8 @@ static float march_one_by_stretch(const OccView& occ, const float* box, const fl
             if (n_desc > 0) lat_anchor(m, table, buf.pend[0]);
             const float anchor = m.t;
             const bool ok = m.ok;
-            float first[HostBuf::K], after[HostBuf::K];
-            uint32_t cnt[HostBuf::K];
+            float first[kSlots], after[kSlots];
+            uint32_t cnt[kSlots];
             for (int j = n_desc - 1; j >= 0; --j)  // any order: here the last one first
                 lat_stretch(L, anchor, ok, buf.pend[j], buf.open[j], first[j], cnt[j], after[j]);
             for (int j = 0; j < n_desc; ++j) {
@@ -191,25 +193,14 @@ static float march_one_by_stretch(const OccView& occ, const float* box, const fl
     return term;
 }
 
-extern "C" {
-
-void sim_by_stretch_counts(long* out, int reset)
-{
-    out[0] = g_by_stretch_rounds;
-    out[1] = g_tables;
-    if (reset) g_by_stretch_rounds = g_tables = 0;
-}
-
-// March all rays; per ray: n_samples, n_runs, terminate plane; runs appended to
-// flat arrays (caller passes capacity; returns total runs or -1 on overflow).
-int64_t sim_march(int32_t n_rays, const float* rays_o, const float* rays_d,
-                  const float* near_planes, const float* far_planes,
-                  int n_grids, int rx, int ry, int rz, const uint64_t* words, const uint32_t* coarse,
-                  const int32_t* bounds, int accel, const float* aabbs,
-                  const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,  // NULL => single level inline
-                  float step_size,
-                  int64_t* n_samples, int64_t* n_runs, float* terminate, int32_t* ok_flags,
-                  float* run_t, uint32_t* run_n, int64_t run_capacity)
+// March all rays with a descriptor buffer of kSlots stretches; see sim_march.
+template <int kSlots>
+static int64_t march_all(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
+                         const float* far_planes, int n_grids, int rx, int ry, int rz, const uint64_t* words,
+                         const uint32_t* coarse, const int32_t* bounds, int accel, const float* aabbs,
+                         const float* t_sorted, const int64_t* t_indices, const uint8_t* hits, float step_size,
+                         int64_t* n_samples, int64_t* n_runs, float* terminate, int32_t* ok_flags, float* run_t,
+                         uint32_t* run_n, int64_t run_capacity)
 {
     OccView occ;
     occ.words = words;
@@ -226,16 +217,17 @@ int64_t sim_march(int32_t n_rays, const float* rays_o, const float* rays_d,
         LatState m;
         float term;
         if (t_sorted == nullptr && accel == 2) {  // accel == 2: phase 2 by stretch, as march_kernel does it for one level
-            term = march_one_by_stretch(occ, aabbs, rays_o + 3 * r, rays_d + 3 * r, near_planes[r], far_planes[r], L, m, vt,
-                                        vn);
+            term = march_one_by_stretch<kSlots>(occ, aabbs, rays_o + 3 * r, rays_d + 3 * r, near_planes[r],
+                                                far_planes[r], L, m, vt, vn);
         } else if (t_sorted == nullptr) {
             SingleBox b{aabbs};
-            term = march_one(b, occ, rays_o + 3 * r, rays_d + 3 * r, near_planes[r], far_planes[r], L, m, vt, vn,
-                             accel);
+            term = march_one<kSlots>(b, occ, rays_o + 3 * r, rays_d + 3 * r, near_planes[r], far_planes[r], L, m, vt,
+                                     vn, accel);
         } else {
             SortedBoxes b{aabbs, n_grids, t_sorted + (int64_t)r * 2 * n_grids, t_indices + (int64_t)r * 2 * n_grids,
                           hits + (int64_t)r * n_grids};
-            term = march_one(b, occ, rays_o + 3 * r, rays_d + 3 * r, near_planes[r], far_planes[r], L, m, vt, vn, 0);
+            term = march_one<kSlots>(b, occ, rays_o + 3 * r, rays_d + 3 * r, near_planes[r], far_planes[r], L, m, vt,
+                                     vn, 0);
         }
         n_samples[r] = m.n_samples;
         n_runs[r] = m.n_runs;
@@ -245,6 +237,54 @@ int64_t sim_march(int32_t n_rays, const float* rays_o, const float* rays_d,
         for (size_t q = 0; q < vt.size(); ++q) { run_t[total] = vt[q]; run_n[total] = vn[q]; ++total; }
     }
     return total;
+}
+
+extern "C" {
+
+void sim_by_stretch_counts(long* out, int reset)
+{
+    out[0] = g_by_stretch_rounds;
+    out[1] = g_tables;
+    if (reset) g_by_stretch_rounds = g_tables = 0;
+}
+
+// March all rays; per ray: n_samples, n_runs, terminate plane; runs appended to
+// flat arrays (caller passes capacity; returns total runs or -1 on overflow).
+// `slots` stretch descriptors are buffered per ray between the two phases: 8 or 16, as the two widths of
+// march_kernel (traverse.cu: kDescSlots / kDescSlotsWide); any other value returns -2.
+int64_t sim_march_slots(int32_t n_rays, const float* rays_o, const float* rays_d,
+                        const float* near_planes, const float* far_planes,
+                        int n_grids, int rx, int ry, int rz, const uint64_t* words, const uint32_t* coarse,
+                        const int32_t* bounds, int accel, const float* aabbs,
+                        const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,  // NULL => single level inline
+                        float step_size,
+                        int64_t* n_samples, int64_t* n_runs, float* terminate, int32_t* ok_flags,
+                        float* run_t, uint32_t* run_n, int64_t run_capacity, int slots)
+{
+    if (slots == 8)
+        return march_all<8>(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, coarse, bounds,
+                            accel, aabbs, t_sorted, t_indices, hits, step_size, n_samples, n_runs, terminate, ok_flags,
+                            run_t, run_n, run_capacity);
+    if (slots == 16)
+        return march_all<16>(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, coarse,
+                             bounds, accel, aabbs, t_sorted, t_indices, hits, step_size, n_samples, n_runs, terminate,
+                             ok_flags, run_t, run_n, run_capacity);
+    return -2;
+}
+
+// the 8-slot march (march_kernel's narrow width)
+int64_t sim_march(int32_t n_rays, const float* rays_o, const float* rays_d,
+                  const float* near_planes, const float* far_planes,
+                  int n_grids, int rx, int ry, int rz, const uint64_t* words, const uint32_t* coarse,
+                  const int32_t* bounds, int accel, const float* aabbs,
+                  const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,
+                  float step_size,
+                  int64_t* n_samples, int64_t* n_runs, float* terminate, int32_t* ok_flags,
+                  float* run_t, uint32_t* run_n, int64_t run_capacity)
+{
+    return sim_march_slots(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, coarse, bounds,
+                           accel, aabbs, t_sorted, t_indices, hits, step_size, n_samples, n_runs, terminate, ok_flags,
+                           run_t, run_n, run_capacity, 8);
 }
 
 

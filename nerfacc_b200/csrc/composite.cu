@@ -7,13 +7,18 @@
 // background blend; a second kernel is the matching backward.
 //
 // Mapping: a ray's samples are contiguous in the packed arrays, so a warp owns a
-// ray and walks it in 32-sample tiles: coalesced loads, a shuffle scan for the
-// segmented exclusive sum / product, per-lane partial sums reduced once per ray.
+// ray and a lane owns a group of 4 consecutive samples (global index 4g .. 4g+3):
+// the warp covers 128 samples per step, each lane scans its group in registers and
+// one shuffle scan joins the lanes; per-lane partial sums are reduced once per ray.
+// Groups are aligned to the ARRAY, not to the ray: the first / last group of a ray
+// may hold samples of its neighbours, which are masked (and written element-wise).
 // No atomics (deterministic, unlike the reference's index_add_), no tensor
 // cores (no contraction here); the kernels are HBM-bound: 44 B/sample forward,
 // 48 B/sample backward (SURVEY.md section 8d).
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "../../include/nerfacc_b200.h"
 #include "sm_count.cuh"
@@ -87,111 +92,257 @@ __device__ __forceinline__ float exp_neg(float x) { return __expf(-x); }
 
 constexpr float kEpsF32 = 1.1920929e-07f;  // torch.finfo(float32).eps, reference volrend.py:158
 
-// per-sample forward quantities for one 32-sample tile of a ray
-template <bool kAlpha>
-struct TileFwd {
-    float delta, mid, a, T, w, x;  // x: sigma*dt (density) or 1-alpha (alpha route)
+// Compile-time specialisation of the forward and backward kernels.
+//   kAlpha: the alpha route (`dens` holds alphas) instead of the density route.
+//   kVec:   every per-sample pointer is 16-byte aligned, so a group that lies inside the array moves as one float4
+//           per array (the 12 colour floats as three).  Otherwise every group is loaded and stored element-wise, as
+//           the array's last partial group always is.  The arithmetic is the same either way, so results do not
+//           depend on where the inputs sit in memory.
+//   kHot:   the training step: density route with colours, no prefix_trans, every forward output; in the backward,
+//           upstream gradients on colours / opacities / depths only; fewer than 2^31 - 8 samples.  Every test of an
+//           optional pointer folds to a constant and indices are 32-bit: these kernels are as much issue-bound as
+//           HBM-bound, so instructions per sample matter.
+template <bool kAlpha_, bool kVec_, bool kHot_ = false>
+struct Cfg {
+    static constexpr bool kAlpha = kAlpha_, kVec = kVec_, kHot = kHot_;
+    using Index = std::conditional_t<kHot, int, int64_t>;
+    // `has`: a pointer every hot call passes; `extra`: one no hot call passes
+    static __device__ __forceinline__ bool has(const void* q) { return kHot || q != nullptr; }
+    static __device__ __forceinline__ bool extra(const void* q) { return !kHot && q != nullptr; }
+};
+using HotCfg = Cfg<false, true, true>;
+
+// Group g (samples 4g .. 4g+3) of a ray [start, end): the samples lo <= e < hi belong to the ray.
+template <class C>
+struct Span {
+    using I = typename C::Index;
+    I g, n_total;
+    int lo, hi;
+    bool valid;  // the group overlaps the ray
+
+    __device__ __forceinline__ Span(I g_, I g_last, I start, I end, I n_total_) : g(g_), n_total(n_total_)
+    {
+        valid = g <= g_last;
+        if constexpr (sizeof(I) == 4) {
+            lo = start - 4 * g;
+            hi = end - 4 * g;
+        } else {  // only how the bounds compare with 0 .. 4 matters: clamp before narrowing
+            lo = (int)max((I)-8, start - 4 * g);
+            hi = (int)min((I)8, end - 4 * g);
+        }
+        if (!valid) lo = 4;
+    }
+    __device__ __forceinline__ bool ok(int e) const { return e >= lo && e < hi; }
+    // The group lies inside the array and moves as float4.  Evaluated where it is used: computed up front, it
+    // leads the compiler to keep one pointer per array live across the loop (10 more registers on the hot path).
+    __device__ __forceinline__ bool full() const { return C::kVec && 4 * g + 3 < n_total; }
+    __device__ __forceinline__ bool all() const { return lo <= 0 && hi >= 4 && full(); }
 };
 
-template <bool kAlpha>
-__device__ __forceinline__ void tile_forward(const CompositeParams& p, int64_t i, bool valid, int lane, float& carry,
-                                             TileFwd<kAlpha>& q)
+// the g-th float4 of `base`
+template <class I>
+__device__ __forceinline__ void ldg4(const float* base, I g, float x[4])
 {
-    float ts = 0.f, te = 0.f, v = 0.f;
-    if (valid) {
-        v = __ldg(p.dens + i);
-        if (p.t_starts) {
-            ts = __ldg(p.t_starts + i);
-            te = __ldg(p.t_ends + i);
-        }
-    }
-    q.delta = te - ts;
-    q.mid = (ts + te) * 0.5f;
-    float T;
-    if (!kAlpha) {
-        // reference volrend.py:271-275
-        const float sd = v * q.delta;
-        const float incl = warp_scan_sum(sd, lane);
-        T = exp_neg(carry + (incl - sd));
-        q.a = 1.0f - exp_neg(sd);
-        q.x = sd;
-        carry += __shfl_sync(kFull, incl, 31);
-    } else {
-        // reference volrend.py:211-213
-        const float om = valid ? 1.0f - v : 1.0f;
-        const float incl = warp_scan_prod(om, lane);
-        float excl = __shfl_up_sync(kFull, incl, 1);
-        if (lane == 0) excl = 1.0f;
-        T = carry * excl;
-        q.a = v;
-        q.x = om;
-        carry *= __shfl_sync(kFull, incl, 31);
-    }
-    if (p.prefix_trans && valid) T *= __ldg(p.prefix_trans + i);
-    q.T = T;
-    q.w = T * q.a;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(base) + g);
+    x[0] = v.x; x[1] = v.y; x[2] = v.z; x[3] = v.w;
 }
 
-template <bool kAlpha>
-__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_fwd_kernel(const CompositeParams p)
+template <class C>
+__device__ __forceinline__ void load4(const float* base, const Span<C>& s, float x[4])
 {
+    if (s.full()) {
+        ldg4(base, s.g, x);
+    } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) x[e] = (4 * s.g + e < s.n_total) ? __ldg(base + 4 * s.g + e) : 0.f;
+    }
+}
+
+template <class C>
+__device__ __forceinline__ void store4(float* base, const Span<C>& s, const float x[4])
+{
+    if (s.all()) {
+        *(reinterpret_cast<float4*>(base) + s.g) = make_float4(x[0], x[1], x[2], x[3]);
+    } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+            if (s.ok(e)) base[4 * s.g + e] = x[e];
+    }
+}
+
+// the inputs of one group; what is absent stays 0 (prefix_trans: 1)
+struct Group {
+    float ts[4], te[4], v[4], pt[4], c[12];
+};
+
+template <class C>
+__device__ __forceinline__ void load_group(const CompositeParams& p, const Span<C>& s, bool colours, Group& h)
+{
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        h.ts[e] = h.te[e] = h.v[e] = 0.f;
+        h.pt[e] = 1.f;
+    }
+#pragma unroll
+    for (int k = 0; k < 12; ++k) h.c[k] = 0.f;
+    if (!s.valid) return;
+    const bool dt = C::has(p.t_starts), pt = C::extra(p.prefix_trans);
+    if (s.full()) {
+        ldg4(p.dens, s.g, h.v);
+        if (dt) {
+            ldg4(p.t_starts, s.g, h.ts);
+            ldg4(p.t_ends, s.g, h.te);
+        }
+        if (pt) ldg4(p.prefix_trans, s.g, h.pt);
+        if (colours) {
+            ldg4(p.rgbs, 3 * s.g, h.c);
+            ldg4(p.rgbs, 3 * s.g + 1, h.c + 4);
+            ldg4(p.rgbs, 3 * s.g + 2, h.c + 8);
+        }
+    } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const auto i = 4 * s.g + e;
+            if (i >= s.n_total) continue;
+            h.v[e] = __ldg(p.dens + i);
+            if (dt) {
+                h.ts[e] = __ldg(p.t_starts + i);
+                h.te[e] = __ldg(p.t_ends + i);
+            }
+            if (pt) h.pt[e] = __ldg(p.prefix_trans + i);
+            if (colours) {
+                h.c[3 * e] = __ldg(p.rgbs + 3 * i);
+                h.c[3 * e + 1] = __ldg(p.rgbs + 3 * i + 1);
+                h.c[3 * e + 2] = __ldg(p.rgbs + 3 * i + 2);
+            }
+        }
+    }
+}
+
+// upstream gradients on the per-sample outputs (0 where absent); unused ones are never loaded
+template <class C>
+__device__ __forceinline__ void load_sample_grads(const CompositeParams& p, const Span<C>& s, float gw[4],
+                                                  float gt[4], float ga[4])
+{
+#pragma unroll
+    for (int e = 0; e < 4; ++e) gw[e] = gt[e] = ga[e] = 0.f;
+    if (!s.valid) return;
+    if (C::extra(p.gW)) load4(p.gW, s, gw);
+    if (C::extra(p.gT)) load4(p.gT, s, gt);
+    if (C::extra(p.gA)) load4(p.gA, s, ga);
+}
+
+// transmittance, alpha and weight of a group's samples; `carry` is what the ray's earlier groups pass on
+struct GroupFwd {
+    float T[4], a[4], w[4], x[4];  // x: sigma*dt (density route) or 1-alpha (alpha route)
+};
+
+template <class C>
+__device__ __forceinline__ void group_forward(const Group& h, const Span<C>& s, int lane, float& carry,
+                                              GroupFwd& q)
+{
+    if constexpr (!C::kAlpha) {
+        // reference volrend.py:271-275
+        float run = 0.f, incl[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            q.x[e] = s.ok(e) ? h.v[e] * (h.te[e] - h.ts[e]) : 0.f;
+            run += q.x[e];
+            incl[e] = run;
+        }
+        const float tot = warp_scan_sum(run, lane);  // inclusive over lanes
+        const float off = carry + (tot - run);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            q.T[e] = exp_neg(off + (incl[e] - q.x[e])) * h.pt[e];
+            q.a[e] = 1.0f - exp_neg(q.x[e]);
+            q.w[e] = q.T[e] * q.a[e];
+        }
+        carry += __shfl_sync(kFull, tot, 31);
+    } else {
+        // reference volrend.py:211-213
+        float run = 1.f, excl[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            q.x[e] = s.ok(e) ? 1.0f - h.v[e] : 1.0f;
+            excl[e] = run;
+            run *= q.x[e];
+        }
+        const float tot = warp_scan_prod(run, lane);
+        float off = __shfl_up_sync(kFull, tot, 1);
+        if (lane == 0) off = 1.0f;
+        off *= carry;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            q.T[e] = off * excl[e] * h.pt[e];
+            q.a[e] = h.v[e];
+            q.w[e] = q.T[e] * q.a[e];
+        }
+        carry *= __shfl_sync(kFull, tot, 31);
+    }
+}
+
+template <class C>
+__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_fwd_kernel(const CompositeParams p,
+                                                                           typename C::Index n_total)
+{
+    using I = typename C::Index;
     const int lane = threadIdx.x & 31;
-    const bool accumulate = p.opac != nullptr || p.colors != nullptr || p.depths != nullptr || p.raw != nullptr;
+    const bool accumulate = C::has(p.opac) || C::has(p.colors) || C::has(p.depths) || C::has(p.raw);
     // persistent warps: ray = global warp id, then stride by the number of warps in the grid
     for (int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); r < p.n_rays; r += gridDim.x * kWarpsPerCta) {
-    const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
-    const int64_t start = pi.x;
-    const int64_t n = pi.y;
-
-    float carry = kAlpha ? 1.0f : 0.0f;
-    float aO = 0.f, aD = 0.f, aC0 = 0.f, aC1 = 0.f, aC2 = 0.f;
-    for (int64_t base = 0; base < n; base += 32) {
-        const int64_t i = start + base + lane;
-        const bool valid = base + lane < n;
-        float c0 = 0.f, c1 = 0.f, c2 = 0.f;
-        if (p.rgbs && valid) {
-            c0 = __ldg(p.rgbs + 3 * i);
-            c1 = __ldg(p.rgbs + 3 * i + 1);
-            c2 = __ldg(p.rgbs + 3 * i + 2);
-        }
-        TileFwd<kAlpha> q;
-        tile_forward<kAlpha>(p, i, valid, lane, carry, q);
-        if (valid) {
-            if (p.weights) p.weights[i] = q.w;
-            if (p.trans) p.trans[i] = q.T;
-            if (p.alphas) p.alphas[i] = q.a;
-            aO += q.w;
-            aD += q.w * q.mid;
-            aC0 += q.w * c0;
-            aC1 += q.w * c1;
-            aC2 += q.w * c2;
-        }
-    }
-    if (!accumulate) continue;
-    aO = warp_sum(aO);
-    aD = warp_sum(aD);
-    aC0 = warp_sum(aC0);
-    aC1 = warp_sum(aC1);
-    aC2 = warp_sum(aC2);
-    if (lane == 0) {
-        if (p.raw) {
-            float* w = p.raw + 5 * (int64_t)r;
-            w[0] = aC0; w[1] = aC1; w[2] = aC2; w[3] = aO; w[4] = aD;
-        }
-        if (p.opac) p.opac[r] = aO;
-        if (p.depths) p.depths[r] = p.expected_depths ? aD / fmaxf(aO, kEpsF32) : aD;
-        if (p.colors) {
-            float b0 = 0.f, b1 = 0.f, b2 = 0.f;
-            if (p.bkgd) {
-                const float k = 1.0f - aO;
-                b0 = p.bkgd[0] * k; b1 = p.bkgd[1] * k; b2 = p.bkgd[2] * k;
+        const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
+        const I start = (I)pi.x, end = (I)(pi.x + pi.y);
+        float carry = C::kAlpha ? 1.0f : 0.0f;
+        float aO = 0.f, aD = 0.f, aC0 = 0.f, aC1 = 0.f, aC2 = 0.f;
+        if (end > start) {
+            const I g_last = (end - 1) >> 2;
+            for (I gb = start >> 2; gb <= g_last; gb += 32) {
+                const Span<C> s(gb + lane, g_last, start, end, n_total);
+                Group h;
+                load_group(p, s, C::has(p.rgbs), h);
+                GroupFwd q;
+                group_forward(h, s, lane, carry, q);
+                if (!s.valid) continue;
+                if (C::has(p.weights)) store4(p.weights, s, q.w);
+                if (C::has(p.trans)) store4(p.trans, s, q.T);
+                if (C::has(p.alphas)) store4(p.alphas, s, q.a);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float w = s.ok(e) ? q.w[e] : 0.f;
+                    aO += w;
+                    aD += w * ((h.ts[e] + h.te[e]) * 0.5f);
+                    aC0 += w * h.c[3 * e];
+                    aC1 += w * h.c[3 * e + 1];
+                    aC2 += w * h.c[3 * e + 2];
+                }
             }
-            p.colors[3 * (int64_t)r + 0] = aC0 + b0;
-            p.colors[3 * (int64_t)r + 1] = aC1 + b1;
-            p.colors[3 * (int64_t)r + 2] = aC2 + b2;
+        }
+        if (!accumulate) continue;
+        aO = warp_sum(aO);
+        aD = warp_sum(aD);
+        aC0 = warp_sum(aC0);
+        aC1 = warp_sum(aC1);
+        aC2 = warp_sum(aC2);
+        if (lane == 0) {
+            if (C::has(p.raw)) {
+                float* w = p.raw + 5 * (int64_t)r;
+                w[0] = aC0; w[1] = aC1; w[2] = aC2; w[3] = aO; w[4] = aD;
+            }
+            if (C::has(p.opac)) p.opac[r] = aO;
+            if (C::has(p.depths)) p.depths[r] = p.expected_depths ? aD / fmaxf(aO, kEpsF32) : aD;
+            if (C::has(p.colors)) {
+                float b0 = 0.f, b1 = 0.f, b2 = 0.f;
+                if (p.bkgd) {
+                    const float k = 1.0f - aO;
+                    b0 = p.bkgd[0] * k; b1 = p.bkgd[1] * k; b2 = p.bkgd[2] * k;
+                }
+                p.colors[3 * (int64_t)r + 0] = aC0 + b0;
+                p.colors[3 * (int64_t)r + 1] = aC1 + b1;
+                p.colors[3 * (int64_t)r + 2] = aC2 + b2;
+            }
         }
     }
-    }  // ray loop
 }
 
 // Backward.  With g_i = dL/dw_i = gC'.c_i + gO' + gD'.m_i + gW_i  (primes: after
@@ -202,591 +353,29 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) composite_fwd_kernel(const 
 //   S_i = sum_{k>i} (g_k w_k + gT_k T_k),     dL/dc_i = w_i gC'
 // S_i is taken as Total - inclusive prefix, so the ray is walked once, forwards,
 // re-computing T/w from the inputs instead of re-reading saved tensors.
-template <bool kAlpha>
-__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_bwd_kernel(const CompositeParams p)
+template <class C>
+__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_bwd_kernel(const CompositeParams p,
+                                                                           typename C::Index n_total)
 {
-    const int lane = threadIdx.x & 31;
-    for (int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); r < p.n_rays; r += gridDim.x * kWarpsPerCta) {
-    const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
-    const int64_t start = pi.x;
-    const int64_t n = pi.y;
-    if (n == 0) continue;
-
-    // upstream per-ray gradients, moved back to the raw sums
-    float gc0 = 0.f, gc1 = 0.f, gc2 = 0.f, go = 0.f, gd = 0.f;
-    if (p.gC) {
-        gc0 = p.gC[3 * (int64_t)r]; gc1 = p.gC[3 * (int64_t)r + 1]; gc2 = p.gC[3 * (int64_t)r + 2];
-    }
-    if (p.gO) go = p.gO[r];
-    if (p.gD) gd = p.gD[r];
-    float rC0 = 0.f, rC1 = 0.f, rC2 = 0.f, rO = 0.f, rD = 0.f;
-    if (p.raw) {
-        const float* w = p.raw + 5 * (int64_t)r;
-        rC0 = w[0]; rC1 = w[1]; rC2 = w[2]; rO = w[3]; rD = w[4];
-    }
-    if (p.bkgd) go -= gc0 * p.bkgd[0] + gc1 * p.bkgd[1] + gc2 * p.bkgd[2];
-    if (p.expected_depths && p.gD) {
-        if (rO > kEpsF32) {
-            go -= gd * rD / (rO * rO);
-            gd = gd / rO;
-        } else {
-            gd = gd / kEpsF32;
-        }
-    }
-    const bool have_rgb = p.rgbs != nullptr && p.gC != nullptr;
-
-    // Total = sum_k (g_k w_k + gT_k T_k)
-    float total;
-    if (p.raw && !p.gW && !p.gT) {
-        total = gc0 * rC0 + gc1 * rC1 + gc2 * rC2 + go * rO + gd * rD;
-    } else {
-        float carry = kAlpha ? 1.0f : 0.0f;
-        float acc = 0.f;
-        for (int64_t base = 0; base < n; base += 32) {
-            const int64_t i = start + base + lane;
-            const bool valid = base + lane < n;
-            TileFwd<kAlpha> q;
-            tile_forward<kAlpha>(p, i, valid, lane, carry, q);
-            if (valid) {
-                float g = go + gd * q.mid;
-                if (have_rgb) g += gc0 * __ldg(p.rgbs + 3 * i) + gc1 * __ldg(p.rgbs + 3 * i + 1) + gc2 * __ldg(p.rgbs + 3 * i + 2);
-                if (p.gW) g += __ldg(p.gW + i);
-                float t = g * q.w;
-                if (p.gT) t += __ldg(p.gT + i) * q.T;
-                acc += t;
-            }
-        }
-        total = warp_sum(acc);
-    }
-
-    float carry = kAlpha ? 1.0f : 0.0f;
-    float pcarry = 0.f;
-    for (int64_t base = 0; base < n; base += 32) {
-        const int64_t i = start + base + lane;
-        const bool valid = base + lane < n;
-        float c0 = 0.f, c1 = 0.f, c2 = 0.f;
-        if (have_rgb && valid) {
-            c0 = __ldg(p.rgbs + 3 * i);
-            c1 = __ldg(p.rgbs + 3 * i + 1);
-            c2 = __ldg(p.rgbs + 3 * i + 2);
-        }
-        TileFwd<kAlpha> q;
-        tile_forward<kAlpha>(p, i, valid, lane, carry, q);
-        float g = 0.f, term = 0.f, ga = 0.f;
-        if (valid) {
-            g = go + gd * q.mid + gc0 * c0 + gc1 * c1 + gc2 * c2;
-            if (p.gW) g += __ldg(p.gW + i);
-            term = g * q.w;
-            if (p.gT) term += __ldg(p.gT + i) * q.T;
-            if (p.gA) ga = __ldg(p.gA + i);
-        }
-        const float incl = warp_scan_sum(term, lane);
-        const float suffix = total - (pcarry + incl);
-        pcarry += __shfl_sync(kFull, incl, 31);
-        if (valid) {
-            float gi;
-            if (!kAlpha) gi = q.delta * ((g * q.T + ga) * (1.0f - q.a) - suffix);
-            else gi = g * q.T + ga - suffix / fmaxf(q.x, 1e-10f);
-            p.g_dens[i] = gi;
-            if (p.g_rgbs) {
-                p.g_rgbs[3 * i + 0] = q.w * gc0;
-                p.g_rgbs[3 * i + 1] = q.w * gc1;
-                p.g_rgbs[3 * i + 2] = q.w * gc2;
-            }
-        }
-    }
-    }  // ray loop
-}
-
-// ---------------------------------------------------------------------------
-// Vectorised variants (all per-sample pointers 16-byte aligned): a lane owns a
-// group of 4 consecutive samples (global index 4g .. 4g+3), so t_starts / t_ends /
-// sigmas move as one float4 and the 12 colour floats as three; the warp covers 128
-// samples per step with 6 x 512-byte coalesced loads in flight.  Groups are aligned
-// to the ARRAY, not to the ray: the first / last group of a ray may hold samples of
-// its neighbours, which are masked (and written back element-wise).
-// ---------------------------------------------------------------------------
-struct Vec4 {
-    float v[4];
-};
-
-__device__ __forceinline__ Vec4 load4(const float* base, int64_t g, bool full, int64_t n_total)
-{
-    Vec4 r;
-    if (full) {
-        const float4 x = __ldg(reinterpret_cast<const float4*>(base) + g);
-        r.v[0] = x.x; r.v[1] = x.y; r.v[2] = x.z; r.v[3] = x.w;
-    } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) r.v[e] = (4 * g + e < n_total) ? __ldg(base + 4 * g + e) : 0.f;
-    }
-    return r;
-}
-
-__device__ __forceinline__ void store4(float* base, int64_t g, const Vec4& x, const bool ok[4], bool all)
-{
-    if (all) {
-        *(reinterpret_cast<float4*>(base) + g) = make_float4(x.v[0], x.v[1], x.v[2], x.v[3]);
-    } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-            if (ok[e]) base[4 * g + e] = x.v[e];
-    }
-}
-
-// forward quantities of one group
-struct GroupFwd {
-    Vec4 delta, mid, a, T, w, x;
-};
-
-template <bool kAlpha>
-__device__ __forceinline__ void group_forward(const CompositeParams& p, int64_t g, bool gvalid, bool full,
-                                              int64_t n_total, const bool ok[4], int lane, float& carry, GroupFwd& q)
-{
-    Vec4 ts, te, v;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) ts.v[e] = te.v[e] = v.v[e] = 0.f;
-    if (gvalid) {
-        v = load4(p.dens, g, full, n_total);
-        if (p.t_starts) {
-            ts = load4(p.t_starts, g, full, n_total);
-            te = load4(p.t_ends, g, full, n_total);
-        }
-    }
-    Vec4 pt;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) pt.v[e] = 1.f;
-    if (p.prefix_trans && gvalid) pt = load4(p.prefix_trans, g, full, n_total);
-    float incl[4];
-    if (!kAlpha) {
-        float run = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            q.delta.v[e] = te.v[e] - ts.v[e];
-            q.mid.v[e] = (ts.v[e] + te.v[e]) * 0.5f;
-            const float sd = ok[e] ? v.v[e] * q.delta.v[e] : 0.f;
-            q.x.v[e] = sd;
-            run += sd;
-            incl[e] = run;
-        }
-        const float tot = warp_scan_sum(run, lane);  // inclusive over lanes
-        const float lane_off = carry + (tot - run);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            q.T.v[e] = exp_neg(lane_off + (incl[e] - q.x.v[e])) * pt.v[e];
-            q.a.v[e] = 1.0f - exp_neg(q.x.v[e]);
-            q.w.v[e] = q.T.v[e] * q.a.v[e];
-        }
-        carry += __shfl_sync(kFull, tot, 31);
-    } else {
-        float run = 1.f;
-        float excl[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            q.delta.v[e] = te.v[e] - ts.v[e];
-            q.mid.v[e] = (ts.v[e] + te.v[e]) * 0.5f;
-            const float om = ok[e] ? 1.0f - v.v[e] : 1.0f;
-            q.x.v[e] = om;
-            excl[e] = run;
-            run *= om;
-        }
-        const float tot = warp_scan_prod(run, lane);
-        float lane_off = __shfl_up_sync(kFull, tot, 1);
-        if (lane == 0) lane_off = 1.0f;
-        lane_off *= carry;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            q.T.v[e] = lane_off * excl[e] * pt.v[e];
-            q.a.v[e] = v.v[e];
-            q.w.v[e] = q.T.v[e] * q.a.v[e];
-        }
-        carry *= __shfl_sync(kFull, tot, 31);
-    }
-}
-
-template <bool kAlpha>
-__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_fwd_vec_kernel(const CompositeParams p, int64_t n_total)
-{
-    const int lane = threadIdx.x & 31;
-    const bool accumulate = p.opac != nullptr || p.colors != nullptr || p.depths != nullptr || p.raw != nullptr;
-    for (int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); r < p.n_rays; r += gridDim.x * kWarpsPerCta) {
-    const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
-    const int64_t start = pi.x, end = pi.x + pi.y;
-    float carry = kAlpha ? 1.0f : 0.0f;
-    float aO = 0.f, aD = 0.f, aC0 = 0.f, aC1 = 0.f, aC2 = 0.f;
-    if (end > start) {
-        const int64_t g_last = (end - 1) >> 2;
-        for (int64_t gb = start >> 2; gb <= g_last; gb += 32) {
-            const int64_t g = gb + lane;
-            const bool gvalid = g <= g_last;
-            const bool full = 4 * g + 3 < n_total;
-            bool ok[4];
-            {
-                const int lo = (int)max((int64_t)-8, start - 4 * g), hi = (int)min((int64_t)8, end - 4 * g);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) ok[e] = gvalid && e >= lo && e < hi;
-            }
-            const bool all = ok[0] && ok[3] && full;
-            float c[12];
-#pragma unroll
-            for (int k = 0; k < 12; ++k) c[k] = 0.f;
-            if (p.rgbs && gvalid) {
-                if (full) {
-                    const float4* src = reinterpret_cast<const float4*>(p.rgbs) + 3 * g;
-                    const float4 x0 = __ldg(src), x1 = __ldg(src + 1), x2 = __ldg(src + 2);
-                    c[0] = x0.x; c[1] = x0.y; c[2] = x0.z; c[3] = x0.w;
-                    c[4] = x1.x; c[5] = x1.y; c[6] = x1.z; c[7] = x1.w;
-                    c[8] = x2.x; c[9] = x2.y; c[10] = x2.z; c[11] = x2.w;
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 12; ++k)
-                        if (4 * g + k / 3 < n_total) c[k] = __ldg(p.rgbs + 12 * g + k);
-                }
-            }
-            GroupFwd q;
-            group_forward<kAlpha>(p, g, gvalid, full, n_total, ok, lane, carry, q);
-            if (gvalid) {
-                if (p.weights) store4(p.weights, g, q.w, ok, all);
-                if (p.trans) store4(p.trans, g, q.T, ok, all);
-                if (p.alphas) store4(p.alphas, g, q.a, ok, all);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float w = ok[e] ? q.w.v[e] : 0.f;
-                    aO += w;
-                    aD += w * q.mid.v[e];
-                    aC0 += w * c[3 * e];
-                    aC1 += w * c[3 * e + 1];
-                    aC2 += w * c[3 * e + 2];
-                }
-            }
-        }
-    }
-    if (!accumulate) continue;
-    aO = warp_sum(aO);
-    aD = warp_sum(aD);
-    aC0 = warp_sum(aC0);
-    aC1 = warp_sum(aC1);
-    aC2 = warp_sum(aC2);
-    if (lane == 0) {
-        if (p.raw) {
-            float* w = p.raw + 5 * (int64_t)r;
-            w[0] = aC0; w[1] = aC1; w[2] = aC2; w[3] = aO; w[4] = aD;
-        }
-        if (p.opac) p.opac[r] = aO;
-        if (p.depths) p.depths[r] = p.expected_depths ? aD / fmaxf(aO, kEpsF32) : aD;
-        if (p.colors) {
-            float b0 = 0.f, b1 = 0.f, b2 = 0.f;
-            if (p.bkgd) {
-                const float k = 1.0f - aO;
-                b0 = p.bkgd[0] * k; b1 = p.bkgd[1] * k; b2 = p.bkgd[2] * k;
-            }
-            p.colors[3 * (int64_t)r + 0] = aC0 + b0;
-            p.colors[3 * (int64_t)r + 1] = aC1 + b1;
-            p.colors[3 * (int64_t)r + 2] = aC2 + b2;
-        }
-    }
-    }  // ray loop
-}
-
-template <bool kAlpha>
-__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_bwd_vec_kernel(const CompositeParams p, int64_t n_total)
-{
-    const int lane = threadIdx.x & 31;
-    for (int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); r < p.n_rays; r += gridDim.x * kWarpsPerCta) {
-    const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
-    const int64_t start = pi.x, end = pi.x + pi.y;
-    if (end <= start) continue;
-
-    float gc0 = 0.f, gc1 = 0.f, gc2 = 0.f, go = 0.f, gd = 0.f;
-    if (p.gC) {
-        gc0 = p.gC[3 * (int64_t)r]; gc1 = p.gC[3 * (int64_t)r + 1]; gc2 = p.gC[3 * (int64_t)r + 2];
-    }
-    if (p.gO) go = p.gO[r];
-    if (p.gD) gd = p.gD[r];
-    float rC0 = 0.f, rC1 = 0.f, rC2 = 0.f, rO = 0.f, rD = 0.f;
-    if (p.raw) {
-        const float* w = p.raw + 5 * (int64_t)r;
-        rC0 = w[0]; rC1 = w[1]; rC2 = w[2]; rO = w[3]; rD = w[4];
-    }
-    if (p.bkgd) go -= gc0 * p.bkgd[0] + gc1 * p.bkgd[1] + gc2 * p.bkgd[2];
-    if (p.expected_depths && p.gD) {
-        if (rO > kEpsF32) {
-            go -= gd * rD / (rO * rO);
-            gd = gd / rO;
-        } else {
-            gd = gd / kEpsF32;
-        }
-    }
-    const bool have_rgb = p.rgbs != nullptr && p.gC != nullptr;
-    const int64_t g_first = start >> 2, g_last = (end - 1) >> 2;
-
-    // the general case (gradients on per-sample outputs) needs the ray total first
-    float total;
-    if (p.raw && !p.gW && !p.gT) {
-        total = gc0 * rC0 + gc1 * rC1 + gc2 * rC2 + go * rO + gd * rD;
-    } else {
-        float carry = kAlpha ? 1.0f : 0.0f;
-        float acc = 0.f;
-        for (int64_t gb = g_first; gb <= g_last; gb += 32) {
-            const int64_t g = gb + lane;
-            const bool gvalid = g <= g_last;
-            const bool full = 4 * g + 3 < n_total;
-            bool ok[4];
-            {
-                const int lo = (int)max((int64_t)-8, start - 4 * g), hi = (int)min((int64_t)8, end - 4 * g);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) ok[e] = gvalid && e >= lo && e < hi;
-            }
-            GroupFwd q;
-            group_forward<kAlpha>(p, g, gvalid, full, n_total, ok, lane, carry, q);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                if (!ok[e]) continue;
-                const int64_t i = 4 * g + e;
-                float gg = go + gd * q.mid.v[e];
-                if (have_rgb) gg += gc0 * __ldg(p.rgbs + 3 * i) + gc1 * __ldg(p.rgbs + 3 * i + 1) + gc2 * __ldg(p.rgbs + 3 * i + 2);
-                if (p.gW) gg += __ldg(p.gW + i);
-                float t = gg * q.w.v[e];
-                if (p.gT) t += __ldg(p.gT + i) * q.T.v[e];
-                acc += t;
-            }
-        }
-        total = warp_sum(acc);
-    }
-
-    float carry = kAlpha ? 1.0f : 0.0f;
-    float pcarry = 0.f;
-    for (int64_t gb = g_first; gb <= g_last; gb += 32) {
-        const int64_t g = gb + lane;
-        const bool gvalid = g <= g_last;
-        const bool full = 4 * g + 3 < n_total;
-        bool ok[4];
-        {
-            const int lo = (int)max((int64_t)-8, start - 4 * g), hi = (int)min((int64_t)8, end - 4 * g);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) ok[e] = gvalid && e >= lo && e < hi;
-        }
-        const bool all = ok[0] && ok[3] && full;
-        float c[12];
-#pragma unroll
-        for (int k = 0; k < 12; ++k) c[k] = 0.f;
-        if (have_rgb && gvalid) {
-            if (full) {
-                const float4* src = reinterpret_cast<const float4*>(p.rgbs) + 3 * g;
-                const float4 x0 = __ldg(src), x1 = __ldg(src + 1), x2 = __ldg(src + 2);
-                c[0] = x0.x; c[1] = x0.y; c[2] = x0.z; c[3] = x0.w;
-                c[4] = x1.x; c[5] = x1.y; c[6] = x1.z; c[7] = x1.w;
-                c[8] = x2.x; c[9] = x2.y; c[10] = x2.z; c[11] = x2.w;
-            } else {
-#pragma unroll
-                for (int k = 0; k < 12; ++k)
-                    if (4 * g + k / 3 < n_total) c[k] = __ldg(p.rgbs + 12 * g + k);
-            }
-        }
-        GroupFwd q;
-        group_forward<kAlpha>(p, g, gvalid, full, n_total, ok, lane, carry, q);
-        Vec4 gw, gt, ga;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) gw.v[e] = gt.v[e] = ga.v[e] = 0.f;
-        if (gvalid) {
-            if (p.gW) gw = load4(p.gW, g, full, n_total);
-            if (p.gT) gt = load4(p.gT, g, full, n_total);
-            if (p.gA) ga = load4(p.gA, g, full, n_total);
-        }
-        float gg[4], incl[4];
-        float run = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            gg[e] = go + gd * q.mid.v[e] + gc0 * c[3 * e] + gc1 * c[3 * e + 1] + gc2 * c[3 * e + 2] + gw.v[e];
-            const float term = ok[e] ? gg[e] * q.w.v[e] + gt.v[e] * q.T.v[e] : 0.f;
-            run += term;
-            incl[e] = run;
-        }
-        const float tot = warp_scan_sum(run, lane);
-        const float lane_off = pcarry + (tot - run);
-        pcarry += __shfl_sync(kFull, tot, 31);
-        if (gvalid) {
-            Vec4 gi;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float suffix = total - (lane_off + incl[e]);
-                if (!kAlpha) gi.v[e] = q.delta.v[e] * ((gg[e] * q.T.v[e] + ga.v[e]) * (1.0f - q.a.v[e]) - suffix);
-                else gi.v[e] = gg[e] * q.T.v[e] + ga.v[e] - suffix / fmaxf(q.x.v[e], 1e-10f);
-            }
-            store4(p.g_dens, g, gi, ok, all);
-            if (p.g_rgbs) {
-                if (all) {
-                    float4* dst = reinterpret_cast<float4*>(p.g_rgbs) + 3 * g;
-                    dst[0] = make_float4(q.w.v[0] * gc0, q.w.v[0] * gc1, q.w.v[0] * gc2, q.w.v[1] * gc0);
-                    dst[1] = make_float4(q.w.v[1] * gc1, q.w.v[1] * gc2, q.w.v[2] * gc0, q.w.v[2] * gc1);
-                    dst[2] = make_float4(q.w.v[2] * gc2, q.w.v[3] * gc0, q.w.v[3] * gc1, q.w.v[3] * gc2);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        if (!ok[e]) continue;
-                        const int64_t i = 4 * g + e;
-                        p.g_rgbs[3 * i + 0] = q.w.v[e] * gc0;
-                        p.g_rgbs[3 * i + 1] = q.w.v[e] * gc1;
-                        p.g_rgbs[3 * i + 2] = q.w.v[e] * gc2;
-                    }
-                }
-            }
-        }
-    }
-    }  // ray loop
-}
-
-// ---------------------------------------------------------------------------
-// Hot-path instantiations: density route, colours present, no prefix_trans, every
-// output requested, fewer than 2^31 samples.  Same mapping as the vector kernels
-// above with everything optional compiled out and 32-bit indexing -- these kernels
-// are as much issue-bound as HBM-bound, so instructions per sample matter.
-// ---------------------------------------------------------------------------
-struct HotGroup {
-    float ts[4], te[4], sg[4], c[12];
-};
-
-__device__ __forceinline__ void hot_load(const CompositeParams& p, int g, bool gvalid, int n_total, HotGroup& h)
-{
-#pragma unroll
-    for (int e = 0; e < 4; ++e) h.ts[e] = h.te[e] = h.sg[e] = 0.f;
-#pragma unroll
-    for (int k = 0; k < 12; ++k) h.c[k] = 0.f;
-    if (!gvalid) return;
-    if (4 * g + 3 < n_total) {
-        const float4 a = __ldg(reinterpret_cast<const float4*>(p.t_starts) + g);
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.t_ends) + g);
-        const float4 d = __ldg(reinterpret_cast<const float4*>(p.dens) + g);
-        const float4* src = reinterpret_cast<const float4*>(p.rgbs) + 3 * g;
-        const float4 x0 = __ldg(src), x1 = __ldg(src + 1), x2 = __ldg(src + 2);
-        h.ts[0] = a.x; h.ts[1] = a.y; h.ts[2] = a.z; h.ts[3] = a.w;
-        h.te[0] = b.x; h.te[1] = b.y; h.te[2] = b.z; h.te[3] = b.w;
-        h.sg[0] = d.x; h.sg[1] = d.y; h.sg[2] = d.z; h.sg[3] = d.w;
-        h.c[0] = x0.x; h.c[1] = x0.y; h.c[2] = x0.z; h.c[3] = x0.w;
-        h.c[4] = x1.x; h.c[5] = x1.y; h.c[6] = x1.z; h.c[7] = x1.w;
-        h.c[8] = x2.x; h.c[9] = x2.y; h.c[10] = x2.z; h.c[11] = x2.w;
-    } else {  // only the last group of the whole array can be partial
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int i = 4 * g + e;
-            if (i < n_total) {
-                h.ts[e] = __ldg(p.t_starts + i);
-                h.te[e] = __ldg(p.t_ends + i);
-                h.sg[e] = __ldg(p.dens + i);
-                h.c[3 * e] = __ldg(p.rgbs + 3 * i);
-                h.c[3 * e + 1] = __ldg(p.rgbs + 3 * i + 1);
-                h.c[3 * e + 2] = __ldg(p.rgbs + 3 * i + 2);
-            }
-        }
-    }
-}
-
-// transmittance / alpha / weight of the 4 samples of a group; `carry` = sigma*dt summed so far on the ray
-__device__ __forceinline__ void hot_forward(const HotGroup& h, int lo, int hi, int lane, float& carry, float T[4],
-                                            float a[4], float w[4])
-{
-    float sd[4], incl[4];
-    float run = 0.f;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        sd[e] = (e >= lo && e < hi) ? h.sg[e] * (h.te[e] - h.ts[e]) : 0.f;
-        run += sd[e];
-        incl[e] = run;
-    }
-    const float tot = warp_scan_sum(run, lane);
-    const float off = carry + (tot - run);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        T[e] = exp_neg(off + (incl[e] - sd[e]));
-        a[e] = 1.0f - exp_neg(sd[e]);
-        w[e] = T[e] * a[e];
-    }
-    carry += __shfl_sync(kFull, tot, 31);
-}
-
-__device__ __forceinline__ void hot_store4(float* base, int g, const float x[4], int lo, int hi, bool all)
-{
-    if (all) {
-        *(reinterpret_cast<float4*>(base) + g) = make_float4(x[0], x[1], x[2], x[3]);
-    } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-            if (e >= lo && e < hi) base[4 * g + e] = x[e];
-    }
-}
-
-__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_fwd_hot_kernel(const CompositeParams p, int n_total)
-{
+    using I = typename C::Index;
     const int lane = threadIdx.x & 31;
     for (int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); r < p.n_rays; r += gridDim.x * kWarpsPerCta) {
         const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
-        const int start = (int)pi.x, end = (int)(pi.x + pi.y);
-        float carry = 0.f, aO = 0.f, aD = 0.f, aC0 = 0.f, aC1 = 0.f, aC2 = 0.f;
-        if (end > start) {
-            const int g_last = (end - 1) >> 2;
-            for (int gb = start >> 2; gb <= g_last; gb += 32) {
-                const int g = gb + lane;
-                const bool gvalid = g <= g_last;
-                const int lo = gvalid ? start - 4 * g : 4, hi = end - 4 * g;  // valid elements: lo <= e < hi
-                HotGroup h;
-                hot_load(p, g, gvalid, n_total, h);
-                float T[4], a[4], w[4];
-                hot_forward(h, lo, hi, lane, carry, T, a, w);
-                if (gvalid) {
-                    const bool all = lo <= 0 && hi >= 4 && 4 * g + 3 < n_total;
-                    hot_store4(p.weights, g, w, lo, hi, all);
-                    hot_store4(p.trans, g, T, lo, hi, all);
-                    hot_store4(p.alphas, g, a, lo, hi, all);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float we = (e >= lo && e < hi) ? w[e] : 0.f;
-                        aO += we;
-                        aD += we * ((h.ts[e] + h.te[e]) * 0.5f);
-                        aC0 += we * h.c[3 * e];
-                        aC1 += we * h.c[3 * e + 1];
-                        aC2 += we * h.c[3 * e + 2];
-                    }
-                }
-            }
-        }
-        aO = warp_sum(aO);
-        aD = warp_sum(aD);
-        aC0 = warp_sum(aC0);
-        aC1 = warp_sum(aC1);
-        aC2 = warp_sum(aC2);
-        if (lane == 0) {
-            float* raw = p.raw + 5 * (int64_t)r;
-            raw[0] = aC0; raw[1] = aC1; raw[2] = aC2; raw[3] = aO; raw[4] = aD;
-            p.opac[r] = aO;
-            p.depths[r] = p.expected_depths ? aD / fmaxf(aO, kEpsF32) : aD;
-            float b0 = 0.f, b1 = 0.f, b2 = 0.f;
-            if (p.bkgd) {
-                const float k = 1.0f - aO;
-                b0 = p.bkgd[0] * k; b1 = p.bkgd[1] * k; b2 = p.bkgd[2] * k;
-            }
-            p.colors[3 * (int64_t)r + 0] = aC0 + b0;
-            p.colors[3 * (int64_t)r + 1] = aC1 + b1;
-            p.colors[3 * (int64_t)r + 2] = aC2 + b2;
-        }
-    }
-}
-
-// backward of the above for upstream gradients on colours / opacities / depths only
-__global__ void __launch_bounds__(kWarpsPerCta * 32) composite_bwd_hot_kernel(const CompositeParams p, int n_total)
-{
-    const int lane = threadIdx.x & 31;
-    for (int r = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); r < p.n_rays; r += gridDim.x * kWarpsPerCta) {
-        const longlong2 pi = *reinterpret_cast<const longlong2*>(p.packed_info + 2 * (int64_t)r);
-        const int start = (int)pi.x, end = (int)(pi.x + pi.y);
+        const I start = (I)pi.x, end = (I)(pi.x + pi.y);
         if (end <= start) continue;
+
+        // upstream per-ray gradients, moved back to the raw sums
         float gc0 = 0.f, gc1 = 0.f, gc2 = 0.f, go = 0.f, gd = 0.f;
         if (p.gC) {
             gc0 = p.gC[3 * (int64_t)r]; gc1 = p.gC[3 * (int64_t)r + 1]; gc2 = p.gC[3 * (int64_t)r + 2];
         }
         if (p.gO) go = p.gO[r];
         if (p.gD) gd = p.gD[r];
-        const float* raw = p.raw + 5 * (int64_t)r;
-        const float rO = raw[3], rD = raw[4];
+        float rC0 = 0.f, rC1 = 0.f, rC2 = 0.f, rO = 0.f, rD = 0.f;
+        if (C::has(p.raw)) {
+            const float* w = p.raw + 5 * (int64_t)r;
+            rC0 = w[0]; rC1 = w[1]; rC2 = w[2]; rO = w[3]; rD = w[4];
+        }
         if (p.bkgd) go -= gc0 * p.bkgd[0] + gc1 * p.bkgd[1] + gc2 * p.bkgd[2];
         if (p.expected_depths && p.gD) {
             if (rO > kEpsF32) {
@@ -796,50 +385,96 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) composite_bwd_hot_kernel(co
                 gd = gd / kEpsF32;
             }
         }
-        const float total = gc0 * raw[0] + gc1 * raw[1] + gc2 * raw[2] + go * rO + gd * rD;
-        float carry = 0.f, pcarry = 0.f;
-        const int g_last = (end - 1) >> 2;
-        for (int gb = start >> 2; gb <= g_last; gb += 32) {
-            const int g = gb + lane;
-            const bool gvalid = g <= g_last;
-            const int lo = gvalid ? start - 4 * g : 4, hi = end - 4 * g;
-            HotGroup h;
-            hot_load(p, g, gvalid, n_total, h);
-            float T[4], a[4], w[4];
-            hot_forward(h, lo, hi, lane, carry, T, a, w);
+        // the hot path loads colours even without gC: they are multiplied by zero
+        const bool have_rgb = C::kHot || (p.rgbs != nullptr && p.gC != nullptr);
+        const I g_first = start >> 2, g_last = (end - 1) >> 2;
+
+        // Total = sum_k (g_k w_k + gT_k T_k): from the saved sums, or with gradients on weights / trans a first pass
+        float total;
+        if (C::has(p.raw) && !C::extra(p.gW) && !C::extra(p.gT)) {
+            total = gc0 * rC0 + gc1 * rC1 + gc2 * rC2 + go * rO + gd * rD;
+        } else {
+            float carry = C::kAlpha ? 1.0f : 0.0f;
+            float acc = 0.f;
+            for (I gb = g_first; gb <= g_last; gb += 32) {
+                const Span<C> s(gb + lane, g_last, start, end, n_total);
+                Group h;
+                load_group(p, s, false, h);  // colours per sample below: as a group they cost 7 more registers
+                GroupFwd q;
+                group_forward(h, s, lane, carry, q);
+                float gw[4], gt[4], ga[4];
+                load_sample_grads(p, s, gw, gt, ga);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    if (!s.ok(e)) continue;
+                    const I i = 4 * s.g + e;
+                    float gg = go + gd * ((h.ts[e] + h.te[e]) * 0.5f);
+                    if (have_rgb)
+                        gg += gc0 * __ldg(p.rgbs + 3 * i) + gc1 * __ldg(p.rgbs + 3 * i + 1) +
+                              gc2 * __ldg(p.rgbs + 3 * i + 2);
+                    if (C::extra(p.gW)) gg += gw[e];
+                    float t = gg * q.w[e];
+                    if (C::extra(p.gT)) t += gt[e] * q.T[e];
+                    acc += t;
+                }
+            }
+            total = warp_sum(acc);
+        }
+
+        float carry = C::kAlpha ? 1.0f : 0.0f;
+        float pcarry = 0.f;
+        for (I gb = g_first; gb <= g_last; gb += 32) {
+            const Span<C> s(gb + lane, g_last, start, end, n_total);
+            Group h;
+            load_group(p, s, have_rgb, h);
+            float gw[4], gt[4], ga[4];
+            load_sample_grads(p, s, gw, gt, ga);
+            GroupFwd q;
+            group_forward(h, s, lane, carry, q);
+            // outside the hot path the per-sample gradients are added whether given or not (0 when absent)
             float gg[4], incl[4];
             float run = 0.f;
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                gg[e] = go + gd * ((h.ts[e] + h.te[e]) * 0.5f) + gc0 * h.c[3 * e] + gc1 * h.c[3 * e + 1] + gc2 * h.c[3 * e + 2];
-                run += (e >= lo && e < hi) ? gg[e] * w[e] : 0.f;
+                gg[e] = go + gd * ((h.ts[e] + h.te[e]) * 0.5f) + gc0 * h.c[3 * e] + gc1 * h.c[3 * e + 1] +
+                        gc2 * h.c[3 * e + 2];
+                if (!C::kHot) gg[e] += gw[e];
+                float term = gg[e] * q.w[e];
+                if (!C::kHot) term += gt[e] * q.T[e];
+                run += s.ok(e) ? term : 0.f;
                 incl[e] = run;
             }
             const float tot = warp_scan_sum(run, lane);
             const float off = pcarry + (tot - run);
             pcarry += __shfl_sync(kFull, tot, 31);
-            if (gvalid) {
-                const bool all = lo <= 0 && hi >= 4 && 4 * g + 3 < n_total;
-                float gi[4];
+            if (!s.valid) continue;
+            float gi[4];
 #pragma unroll
-                for (int e = 0; e < 4; ++e)
-                    gi[e] = (h.te[e] - h.ts[e]) * (gg[e] * T[e] * (1.0f - a[e]) - (total - (off + incl[e])));
-                hot_store4(p.g_dens, g, gi, lo, hi, all);
-                if (all) {
-                    float4* dst = reinterpret_cast<float4*>(p.g_rgbs) + 3 * g;
-                    dst[0] = make_float4(w[0] * gc0, w[0] * gc1, w[0] * gc2, w[1] * gc0);
-                    dst[1] = make_float4(w[1] * gc1, w[1] * gc2, w[2] * gc0, w[2] * gc1);
-                    dst[2] = make_float4(w[2] * gc2, w[3] * gc0, w[3] * gc1, w[3] * gc2);
+            for (int e = 0; e < 4; ++e) {
+                const float suffix = total - (off + incl[e]);
+                if constexpr (!C::kAlpha) {
+                    float gT = gg[e] * q.T[e];
+                    if (!C::kHot) gT += ga[e];
+                    gi[e] = (h.te[e] - h.ts[e]) * (gT * (1.0f - q.a[e]) - suffix);
                 } else {
+                    gi[e] = gg[e] * q.T[e] + ga[e] - suffix / fmaxf(q.x[e], 1e-10f);
+                }
+            }
+            store4(p.g_dens, s, gi);
+            if (!C::has(p.g_rgbs)) continue;
+            if (s.all()) {
+                float4* dst = reinterpret_cast<float4*>(p.g_rgbs) + 3 * s.g;
+                dst[0] = make_float4(q.w[0] * gc0, q.w[0] * gc1, q.w[0] * gc2, q.w[1] * gc0);
+                dst[1] = make_float4(q.w[1] * gc1, q.w[1] * gc2, q.w[2] * gc0, q.w[2] * gc1);
+                dst[2] = make_float4(q.w[2] * gc2, q.w[3] * gc0, q.w[3] * gc1, q.w[3] * gc2);
+            } else {
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        if (e >= lo && e < hi) {
-                            const int i = 4 * g + e;
-                            p.g_rgbs[3 * i + 0] = w[e] * gc0;
-                            p.g_rgbs[3 * i + 1] = w[e] * gc1;
-                            p.g_rgbs[3 * i + 2] = w[e] * gc2;
-                        }
-                    }
+                for (int e = 0; e < 4; ++e) {
+                    if (!s.ok(e)) continue;
+                    const I i = 4 * s.g + e;
+                    p.g_rgbs[3 * i + 0] = q.w[e] * gc0;
+                    p.g_rgbs[3 * i + 1] = q.w[e] * gc1;
+                    p.g_rgbs[3 * i + 2] = q.w[e] * gc2;
                 }
             }
         }
@@ -935,6 +570,13 @@ static inline int32_t launch_status_c()
     return e == cudaSuccess ? NFA_OK : (int32_t)e;
 }
 
+template <class I>
+static inline void launch(void (*kernel)(CompositeParams, I), const CompositeParams& p, int32_t n_rays,
+                          int64_t n_samples, cudaStream_t s)
+{
+    kernel<<<persistent_grid(kernel, n_rays), kWarpsPerCta * 32, 0, s>>>(p, (I)n_samples);
+}
+
 extern "C" {
 
 int32_t nfa_composite_fwd(int32_t n_rays, int64_t n_samples, const int64_t* packed_info, const float* t_starts,
@@ -969,20 +611,15 @@ int32_t nfa_composite_fwd(int32_t n_rays, int64_t n_samples, const int64_t* pack
     p.raw = raw;
     const uintptr_t al = (uintptr_t)t_starts | (uintptr_t)t_ends | (uintptr_t)sigmas_or_alphas | (uintptr_t)rgbs |
                          (uintptr_t)prefix_trans | (uintptr_t)weights | (uintptr_t)trans | (uintptr_t)alphas;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int threads = kWarpsPerCta * 32;
+    const cudaStream_t s = (cudaStream_t)stream;
     const bool aligned = (al & 15u) == 0 && n_samples > 0;
     const bool hot = aligned && !from_alpha && rgbs && !prefix_trans && weights && trans && alphas && colors &&
                      opacities && depths && raw && n_samples < (int64_t)0x7fffffff - 8;
-    if (hot) {
-        composite_fwd_hot_kernel<<<persistent_grid(composite_fwd_hot_kernel, n_rays), threads, 0, s>>>(p, (int)n_samples);
-    } else if (aligned) {  // 128-bit path, every option
-        if (from_alpha) composite_fwd_vec_kernel<true><<<persistent_grid(composite_fwd_vec_kernel<true>, n_rays), threads, 0, s>>>(p, n_samples);
-        else composite_fwd_vec_kernel<false><<<persistent_grid(composite_fwd_vec_kernel<false>, n_rays), threads, 0, s>>>(p, n_samples);
-    } else {
-        if (from_alpha) composite_fwd_kernel<true><<<persistent_grid(composite_fwd_kernel<true>, n_rays), threads, 0, s>>>(p);
-        else composite_fwd_kernel<false><<<persistent_grid(composite_fwd_kernel<false>, n_rays), threads, 0, s>>>(p);
-    }
+    if (hot) launch(composite_fwd_kernel<HotCfg>, p, n_rays, n_samples, s);
+    else if (aligned && from_alpha) launch(composite_fwd_kernel<Cfg<true, true>>, p, n_rays, n_samples, s);
+    else if (aligned) launch(composite_fwd_kernel<Cfg<false, true>>, p, n_rays, n_samples, s);
+    else if (from_alpha) launch(composite_fwd_kernel<Cfg<true, false>>, p, n_rays, n_samples, s);
+    else launch(composite_fwd_kernel<Cfg<false, false>>, p, n_rays, n_samples, s);
     return launch_status_c();
 }
 
@@ -1023,20 +660,15 @@ int32_t nfa_composite_bwd(int32_t n_rays, int64_t n_samples, const int64_t* pack
     const uintptr_t al = (uintptr_t)t_starts | (uintptr_t)t_ends | (uintptr_t)sigmas_or_alphas | (uintptr_t)rgbs |
                          (uintptr_t)prefix_trans | (uintptr_t)g_weights | (uintptr_t)g_trans | (uintptr_t)g_alphas |
                          (uintptr_t)g_in | (uintptr_t)g_rgbs;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int threads = kWarpsPerCta * 32;
+    const cudaStream_t s = (cudaStream_t)stream;
     const bool aligned = (al & 15u) == 0 && n_samples > 0;
     const bool hot = aligned && !from_alpha && rgbs && g_rgbs && raw && !prefix_trans && !g_weights && !g_trans &&
                      !g_alphas && n_samples < (int64_t)0x7fffffff - 8;
-    if (hot) {
-        composite_bwd_hot_kernel<<<persistent_grid(composite_bwd_hot_kernel, n_rays), threads, 0, s>>>(p, (int)n_samples);
-    } else if (aligned) {  // 128-bit path, every option
-        if (from_alpha) composite_bwd_vec_kernel<true><<<persistent_grid(composite_bwd_vec_kernel<true>, n_rays), threads, 0, s>>>(p, n_samples);
-        else composite_bwd_vec_kernel<false><<<persistent_grid(composite_bwd_vec_kernel<false>, n_rays), threads, 0, s>>>(p, n_samples);
-    } else {
-        if (from_alpha) composite_bwd_kernel<true><<<persistent_grid(composite_bwd_kernel<true>, n_rays), threads, 0, s>>>(p);
-        else composite_bwd_kernel<false><<<persistent_grid(composite_bwd_kernel<false>, n_rays), threads, 0, s>>>(p);
-    }
+    if (hot) launch(composite_bwd_kernel<HotCfg>, p, n_rays, n_samples, s);
+    else if (aligned && from_alpha) launch(composite_bwd_kernel<Cfg<true, true>>, p, n_rays, n_samples, s);
+    else if (aligned) launch(composite_bwd_kernel<Cfg<false, true>>, p, n_rays, n_samples, s);
+    else if (from_alpha) launch(composite_bwd_kernel<Cfg<true, false>>, p, n_rays, n_samples, s);
+    else launch(composite_bwd_kernel<Cfg<false, false>>, p, n_rays, n_samples, s);
     return launch_status_c();
 }
 

@@ -1,5 +1,11 @@
 """Kernel-level timing of the two fused compositing kernels on config 2 (8.5 M samples, 65536 rays), CUDA events,
-L2 flushed between launches: the launches bench.py's roofline section makes, on their own."""
+L2 flushed between launches: the launches bench.py's roofline section makes, on their own.
+
+    python scripts/composite_probe.py [REPS] [--offset K]
+
+--offset K (1..3) stores every per-sample input and output K float32 elements past a 16-byte boundary, which
+takes the element-wise kernels instead of the hot ones."""
+import argparse
 import json
 import os
 import sys
@@ -12,7 +18,11 @@ import nerfacc_b200 as nfa  # noqa: E402
 from nerfacc_b200 import _lib, scenes  # noqa: E402
 
 dev = torch.device("cuda:0")
-reps = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+ap = argparse.ArgumentParser()
+ap.add_argument("reps", nargs="?", type=int, default=20)
+ap.add_argument("--offset", type=int, default=0, choices=range(4))
+args = ap.parse_args()
+reps = args.reps
 R = 65536
 ro, rd = scenes.ball_rays(R)
 est = nfa.OccGridEstimator(torch.from_numpy(scenes.ROI_AABB), resolution=128).to(dev)
@@ -21,10 +31,20 @@ ri, ts, te = est.sampling(torch.from_numpy(ro).to(dev), torch.from_numpy(rd).to(
 N = ri.numel()
 pi = nfa.pack_info(ri, R)
 f32 = dict(dtype=torch.float32, device=dev)
+
+
+def place(t):  # a copy of t starting args.offset elements into its buffer
+    buf = torch.empty(t.numel() + args.offset, **f32)
+    v = buf[args.offset:].view(t.shape)
+    v.copy_(t)
+    return v
+
+
 sg, cl, gcol = 5 * torch.rand(N, **f32), torch.rand(N, 3, **f32), torch.rand(R, 3, **f32)
-w_o, t_o, a_o = torch.empty(N, **f32), torch.empty(N, **f32), torch.empty(N, **f32)
+ts, te, sg, cl = place(ts), place(te), place(sg), place(cl)
+w_o, t_o, a_o = place(torch.empty(N, **f32)), place(torch.empty(N, **f32)), place(torch.empty(N, **f32))
 c_o, o_o, d_o, raw = torch.empty((R, 3), **f32), torch.empty((R, 1), **f32), torch.empty((R, 1), **f32), torch.empty((R, 5), **f32)
-g_sg, g_cl = torch.empty(N, **f32), torch.empty((N, 3), **f32)
+g_sg, g_cl = place(torch.empty(N, **f32)), place(torch.empty((N, 3), **f32))
 P = _lib.ptr
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 
@@ -54,5 +74,5 @@ def timed(fn):
     return {"median_us": round(tot[len(tot) // 2], 1), "min_us": round(tot[0], 1)}
 
 
-print(json.dumps({"n_samples": N, "composite_fwd": timed(k_fwd), "composite_bwd": timed(k_bwd),
+print(json.dumps({"n_samples": N, "offset": args.offset, "composite_fwd": timed(k_fwd), "composite_bwd": timed(k_bwd),
                   "checksum": [float(c_o.double().sum()), float(g_sg.double().sum())]}))

@@ -591,9 +591,9 @@ def _alpha_grad_f64(alphas, pi, rgb, mids, gC, gO, gD, gW):
 @pytest.mark.gpu
 def test_compositing_tiers_past_resident_warps(orc):
     """One warp per ray in a persistent grid capped at the resident CTAs: with more rays than 64 warps per SM, every
-    warp takes a second ray.  Each kernel tier at that size -- hot (density, every output), vec (alpha route, density
-    with prefix_trans, gradients on weights / trans / alphas), scalar (4-byte-offset views, both routes) -- vs the
-    float64 oracle at the bars of the small-batch tests."""
+    warp takes a second ray.  Each kernel instantiation at that size -- hot (density, every output), vec (alpha route,
+    density with prefix_trans, gradients on weights / trans / alphas), element-wise (4-byte-offset views, both
+    routes) -- vs the float64 oracle at the bars of the small-batch tests."""
     import nerfacc_b200 as nfa
     from nerfacc_b200 import _lib
     R = COMPOSITE_R
@@ -641,7 +641,7 @@ def test_compositing_tiers_past_resident_warps(orc):
     gs, _ = orc.composite_backward(N(ts0), N(te0), N(sig0), None, npi, gW=N(gW), gT=N(gT), gA=N(gA), prefix_trans=N(pt0))
     np.testing.assert_allclose(N(sig.grad), gs, atol=1e-5, rtol=1e-4, err_msg="vec prefix_trans g_sigmas")
 
-    # vec and scalar: the alpha route (and the density route on unaligned views), gradients on the extras too
+    # vec and element-wise: the alpha route (and the density route on unaligned views), gradients on the extras too
     for off in (0, 1):
         ts, te = place(ts0, off), place(te0, off)
         assert (ts.data_ptr() % 16 != 0) == bool(off)

@@ -294,14 +294,14 @@ def test_fused_rendering_vs_oracle(orc, expected_depths, bkgd):
 
 
 def test_vector_and_scalar_kernels_agree(orc):
-    """16-byte aligned inputs take the 128-bit kernels, anything else the scalar ones; both must match the oracle.
-    Also ragged rays: empty rays, 1-sample rays, rays that start / end mid-group."""
+    """16-byte aligned inputs take the 128-bit kernels, anything else the element-wise ones; both must match the
+    oracle.  Also ragged rays: empty rays, 1-sample rays, rays that start / end mid-group."""
     g = torch.Generator().manual_seed(9)
     cnts = torch.tensor([0, 1, 3, 4, 5, 0, 127, 128, 129, 2, 0, 0, 33, 64, 1, 7, 250, 0, 31], dtype=torch.int64)
     starts = torch.cumsum(cnts, 0) - cnts
     pi = torch.stack([starts, cnts], -1).to(dev)
     n, R = int(cnts.sum()), len(cnts)
-    for off in (0, 1):  # off=1: views with a 4-byte offset -> scalar kernels
+    for off in (0, 1):  # off=1: views with a 4-byte offset -> element-wise kernels
         def place(t):  # copy into a view whose storage offset is `off` elements (4 bytes): not 16-byte aligned
             buf = torch.empty((t.shape[0] + off,) + tuple(t.shape[1:]), device=dev)
             v = buf[off:]

@@ -28,7 +28,7 @@ extern "C" {
 #define NFA_ERR_ARG (-1)         /* null pointer / negative size / inconsistent sizes */
 #define NFA_ERR_UNSUPPORTED (-2) /* valid request outside what this build implements */
 
-#define NFA_ABI_VERSION 11
+#define NFA_ABI_VERSION 12
 
 typedef void* nfa_stream_t; /* cudaStream_t */
 
@@ -148,6 +148,35 @@ int32_t nfa_expand_intervals(int32_t n_rays, int64_t run_capacity, const void* w
                              uint8_t* iv_is_left, uint8_t* iv_is_right,
                              int64_t* sm_packed_info, float* sm_vals, int64_t* sm_ray_indices,
                              uint8_t* sm_is_valid, nfa_stream_t stream);
+
+/* ----------------------------------------------------------------------- */
+/* Grid traversal, growing step (cone_angle > 0, step_size > 0)             */
+/* ----------------------------------------------------------------------- */
+
+/* replaces: traverse_grids(..., cone_angle > 0) nerfacc/cuda/csrc/grid.cu:68-282 (launches :320-474) followed by
+ *   `vals[is_left]`, `vals[is_right]` of nerfacc/estimators/occ_grid.py:174-177 -- OccGridEstimator.sampling for
+ *   unbounded scenes, where the step grows with the distance: dt = clamp(t * cone_angle, step_size, 1e10).
+ *
+ * nfa_march_cone: one thread per ray marches sample by sample in the reference's order of operations and appends
+ *   every run (t_first, n) of consecutive samples to the run pool of `workspace`, in nfa_march's record format, with
+ *   nfa_march's per-ray counts, tile sums and totals (so nfa_march_workspace_bytes sizes the workspace and the
+ *   run-pool overflow rule is the same).  Arguments as nfa_march, plus `coarse` (nfa_occ_pack) and cone_angle; no
+ *   terminate planes.  A ray whose marching variable stops advancing (t + dt == t) ends there without an error, as in
+ *   nfa_traverse_generic: totals[3] is always 0.
+ * nfa_expand_cone_samples: runs -> packed (ray_indices, t_starts, t_ends) + packed_info, each run replayed as
+ *   t_{j+1} = t_j + dt(t_j) from its t_first (the same float operations as the march, so the same bits).  Same
+ *   arguments and capacity rule as nfa_expand_samples, plus cone_angle; packed_info is always written. */
+int32_t nfa_march_cone(int32_t n_rays, const float* rays_o, const float* rays_d,
+                       const float* near_planes, const float* far_planes, float near_plane, float far_plane,
+                       int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
+                       const uint64_t* words, const uint32_t* coarse, const float* aabbs,
+                       const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,
+                       float step_size, float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
+                       int64_t* totals_host, nfa_stream_t stream);
+int32_t nfa_expand_cone_samples(int32_t n_rays, int64_t run_capacity, const void* workspace,
+                                const int64_t* totals, float step_size, float cone_angle, int64_t capacity,
+                                int64_t* packed_info, int64_t* ray_indices, float* t_starts, float* t_ends,
+                                nfa_stream_t stream);
 
 /* nfa_traverse_generic: the remaining modes of traverse_grids (nerfacc.cpp:75-96, grid.cu:320-474) --
  *   cone_angle > 0, step_size <= 0 (one sample per occupied cell), traverse_steps_limit, over_allocate

@@ -40,6 +40,11 @@ SIGNATURES = {
     "nfa_expand_samples": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr,
                                     _c_ptr]),
     "nfa_expand_intervals": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_i64] + [_c_ptr] * 10),
+    "nfa_march_cone": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i32, _c_i32, _c_i32, _c_i32,
+                                _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i64, _c_ptr, _c_ptr,
+                                _c_ptr, _c_ptr]),
+    "nfa_expand_cone_samples": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i64, _c_ptr, _c_ptr, _c_ptr,
+                                         _c_ptr, _c_ptr]),
     "nfa_traverse_generic": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_i32, _c_i32, _c_i32, _c_i32,
                                       _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i32, _c_i32]
                              + [_c_ptr] * 14),
@@ -72,7 +77,7 @@ SIGNATURES = {
     "nfa_pack_info": (_c_i32, [_c_i64, _c_ptr, _c_i32, _c_ptr, _c_ptr, _c_ptr]),
 }
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 _lib = None
 launches = 0  # number of native kernel-launching calls made through this module (bench.py reports it)

@@ -5,6 +5,8 @@
 // (/root/reference/nerfacc/cuda/csrc/grid.cu:68-282, launches :364-470).  One thread marches one
 // ray sample by sample, in the reference's order of operations; a first pass counts, a second
 // fills at the scanned offsets (or one pass into fixed-stride slots when over-allocating).
+// The same walk with a run sink (RunSink) feeds nfa_march_cone / nfa_expand_cone_samples, the growing-step
+// sampling path: runs instead of samples, one pass, replayed by the expand kernel.
 // Reuses the DDA set-up, slab test, occupancy words and crossing iterators of march.cuh.
 // Host+device so that tests/host_sim can check it against the oracle on the CPU.
 #pragma once
@@ -87,10 +89,98 @@ NFA_HD void generic_emit(GenericOut& o, float t_last, float t_next, bool continu
     o.n_samples += 1;
 }
 
-// March one ray.  Returns the terminate plane (reference grid.cu:274-275).
-template <class Boxes>
+// Run sink (nfa_march_cone): the samples of a ray as runs -- maximal chains of samples emitted with `continuous`
+// set, each sample starting where the previous one ended.  An emission with `continuous == false` opens a run and
+// the continuous ones that follow extend it; `continuous` is not reset between grid levels, so a run can span
+// levels.  Inside a run every sample is [t, cone_next(t)] of the previous sample's end (the emission loop below
+// computes t_next = t_last + step_length(t_last) and nothing else moves t_last between two such emissions), so a run
+// is fully described by (t_first, n) and cone_expand_run() replays it bit for bit.  Closed runs go to
+// `pool.put(sample_off, n, t_first, run_idx)`.
+template <class Pool>
+struct RunSink {
+    Pool pool;
+    int64_t n_samples;   // samples of the ray so far (generic_march_ray's step limit reads it)
+    uint32_t n_runs;     // runs closed so far
+    uint32_t run_off;    // samples of the ray before the open run
+    uint32_t run_n;      // samples in the open run; 0: none open
+    float run_first;     // start of the open run's first sample
+};
+
+template <class Pool>
+NFA_HD void run_sink_init(RunSink<Pool>& o)
+{
+    o.n_samples = 0;
+    o.n_runs = 0;
+    o.run_off = 0;
+    o.run_n = 0;
+    o.run_first = 0.f;
+}
+
+// hand the open run (if any) to the pool; called by the next opening emission and once at the end of the ray
+template <class Pool>
+NFA_HD void run_sink_close(RunSink<Pool>& o)
+{
+    if (o.run_n == 0u) return;
+    o.pool.put(o.run_off, o.run_n, o.run_first, o.n_runs);
+    o.n_runs += 1;
+    o.run_n = 0;
+}
+
+template <class Pool>
+NFA_HD void generic_emit(RunSink<Pool>& o, float t_last, float t_next, bool continuous)
+{
+    (void)t_next;  // implied by t_last: see RunSink
+    if (!continuous) {
+        run_sink_close(o);
+        o.run_off = (uint32_t)o.n_samples;
+        o.run_first = t_last;
+    }
+    o.run_n += 1;
+    o.n_samples += 1;
+}
+
+// The end of a sample that starts at t inside a run (reference grid.cu:215,259 with step_size > 0).
+NFA_HD float cone_next(float t, float cone, float step) { return f_add(t, step_length(t, cone, step)); }
+
+// The start of the sample j places after the one that starts at t, inside a run.
+NFA_HD float cone_advance(float t, uint32_t j, float cone, float step)
+{
+    for (uint32_t s = 0; s < j; ++s) t = cone_next(t, cone, step);
+    return t;
+}
+
+// Replay the run (t_first, n) into samples k0 .. k0 + n - 1 of the output arrays, none at or past `capacity`, in
+// the order expand_cone_kernel uses: pieces of kExpandLanes samples, sample j of a piece computed by `lane` j from
+// the piece's start, the next piece starting at the end of the last sample.
+constexpr uint32_t kExpandLanes = 32;
+
+NFA_HD void cone_expand_run(float t_first, uint32_t n, float cone, float step, int64_t ray, int64_t k0,
+                            int64_t capacity, int64_t* ray_indices, float* t_starts, float* t_ends)
+{
+    float t = t_first;
+    for (uint32_t base = 0; base < n; base += kExpandLanes) {
+        const uint32_t m = n - base < kExpandLanes ? n - base : kExpandLanes;
+        float last = t;
+        for (uint32_t lane = 0; lane < m; ++lane) {
+            const float ts = cone_advance(t, lane, cone, step);
+            const float te = cone_next(ts, cone, step);
+            const int64_t k = k0 + base + lane;
+            if (k < capacity) {
+                ray_indices[k] = ray;
+                t_starts[k] = ts;
+                t_ends[k] = te;
+            }
+            last = te;
+        }
+        t = last;
+    }
+}
+
+// March one ray into the sink `out` (GenericOut or RunSink).  Returns the terminate plane (reference
+// grid.cu:274-275).
+template <class Boxes, class Out>
 NFA_HD float generic_march_ray(const Boxes& boxes, const OccView& occ, const float o[3], const float d[3],
-                               float near, float far, float step, float cone, int32_t limit, GenericOut& out)
+                               float near, float far, float step, float cone, int32_t limit, Out& out)
 {
     Walk w;  // only the ray fields + segment iterator are used here
     walk_init(w, o, d, near, far);

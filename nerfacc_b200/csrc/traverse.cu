@@ -21,11 +21,16 @@
 //                     closed form (expand.cuh) and store them coalesced, 128-bit stores
 //                     when the outputs are 16-byte aligned; the <true> flavour writes the
 //                     interval-edge form traverse_grids() returns.
+//   march_cone_kernel / expand_cone_kernel
+//                     sampling() with growing steps (cone_angle > 0): 1 thread / ray walks sample by sample
+//                     (march_generic.cuh) into the same run pool, counts and tile sums as march_kernel;
+//                     a warp replays 32 runs one after the other, one lane per sample of a 32-sample piece.
 //   generic_traverse_kernel  every other traverse_grids mode (march_generic.cuh).
 //   ray_aabb_kernel / intersect_sorted_kernel  slab tests (+ sorted crossings of nested boxes).
 //
 // No tensor cores: the path has no dense contraction; it is bound by dependent
 // f32 chains (march) and by HBM stores (expand).  See DESIGN.md.
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -37,6 +42,8 @@
 #include "occ_pack.cuh"
 
 namespace nfa {
+
+namespace cg = cooperative_groups;
 
 constexpr int kMaxTileRays = 512;   // rays per CTA in the march / offsets kernels: march_tile_rays(), <= this
 constexpr int kDescSlots = 8;       // stretch descriptors buffered per ray between the two march phases ...
@@ -288,14 +295,138 @@ __host__ __device__ inline size_t march_smem_bytes(int tile, int slots)
     return (size_t)tile * 4 * (3 + 3 + 2 * slots + 1);
 }
 
+// ---------------------------------------------------------------------------
+// end of a march CTA (march_kernel, march_cone_kernel): tile sums, every ray's sample offset inside its tile and, in
+// the last CTA to finish, the tile bases and the grand totals
+// ---------------------------------------------------------------------------
+// Thread `threadIdx.x` holds ray r0 + rt (`active`: it has one) and that ray's counts; `s_cnt` is tile u32 of shared
+// memory the CTA no longer uses.  Returns true in every thread of the last CTA to finish.
+__device__ __forceinline__ bool march_tile_sums(const Workspace& ws, int r0, int nr, int rt, bool active,
+                                                uint32_t n_samples, uint32_t n_runs, bool stuck, uint32_t* s_cnt)
+{
+    __shared__ unsigned long long s_red_samples[kMaxTileRays / 32];
+    __shared__ uint32_t s_red_runs[kMaxTileRays / 32], s_red_flags[kMaxTileRays / 32], s_wsum[kMaxTileRays / 32];
+    __shared__ bool s_last;
+    const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31;
+    const int n_warps = T >> 5;
+    unsigned long long vs = active ? n_samples : 0u;
+    uint32_t vr = active ? n_runs : 0u, vf = (active && stuck) ? 1u : 0u;
+#pragma unroll
+    for (int sft = 16; sft > 0; sft >>= 1) {
+        vs += __shfl_xor_sync(0xffffffffu, vs, sft);
+        vr += __shfl_xor_sync(0xffffffffu, vr, sft);
+        vf += __shfl_xor_sync(0xffffffffu, vf, sft);
+    }
+    if (lane == 0) {
+        s_red_samples[tid >> 5] = vs;
+        s_red_runs[tid >> 5] = vr;
+        s_red_flags[tid >> 5] = vf;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        TileSum ts;
+        ts.samples = 0;
+        ts.runs = 0;
+        ts.stuck = 0;
+        for (int k = 0; k < n_warps; ++k) {
+            ts.samples += s_red_samples[k];
+            ts.runs += s_red_runs[k];
+            ts.stuck += s_red_flags[k];
+        }
+        ws.tiles[blockIdx.x] = ts;
+        __threadfence();
+        const uint32_t prev = atomicAdd(ws.done, 1u);
+        s_last = (prev == (uint32_t)(gridDim.x - 1));
+    }
+    // Samples of the earlier rays of this tile, in RAY order (march_kernel's threads hold the rays in sorted order):
+    // with the tile bases below this is every ray's packed_info start, so that no separate offsets pass has to run
+    // before the samples are expanded.
+    if (active) s_cnt[rt] = n_samples;
+    __syncthreads();
+    {
+        const uint32_t cs = tid < nr ? s_cnt[tid] : 0u;
+        uint32_t xs = cs;
+#pragma unroll
+        for (int sft = 1; sft < 32; sft <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xffffffffu, xs, sft);
+            if (lane >= sft) xs += y;
+        }
+        if (lane == 31) s_wsum[tid >> 5] = xs;
+        __syncthreads();
+        uint32_t before = xs - cs;
+        for (int k = 0; k < (tid >> 5); ++k) before += s_wsum[k];
+        if (tid < nr) ws.loc_samples[r0 + tid] = before;
+    }
+    return s_last;
+}
+
+// Last CTA only: tile bases (exclusive scan of the tile sums: a contiguous chunk of tiles per thread) and the totals
+//   [0] samples, [1] runs, [2] run-pool capacity used for this call, [3] stuck rays
+// to `totals` and, if given, the pinned host mirror `totals_host`; leaves the workspace header zero (reusable).
+__device__ __forceinline__ void march_totals(const Workspace& ws, int64_t* totals, int64_t* totals_host)
+{
+    __shared__ unsigned long long s_tot[3][kMaxTileRays / 32];
+    const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31;
+    const int n_warps = T >> 5;
+    __threadfence();
+    const int n_tiles = ws.n_tiles;
+    const int chunk = (n_tiles + T - 1) / T;
+    const int i0 = min(tid * chunk, n_tiles), i1 = min(i0 + chunk, n_tiles);
+    unsigned long long a = 0, b = 0, c = 0;
+    for (int i = i0; i < i1; ++i) {
+        const volatile unsigned long long* q = (const volatile unsigned long long*)&ws.tiles[i];
+        const unsigned long long w0 = q[0], w1 = q[1];  // {samples}, {runs | stuck << 32}
+        a += w0;
+        b += (uint32_t)w1;
+        c += w1 >> 32;
+    }
+    unsigned long long xa = a;
+#pragma unroll
+    for (int sft = 1; sft < 32; sft <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, xa, sft);
+        if (lane >= sft) xa += y;
+    }
+#pragma unroll
+    for (int sft = 16; sft > 0; sft >>= 1) {
+        b += __shfl_xor_sync(0xffffffffu, b, sft);
+        c += __shfl_xor_sync(0xffffffffu, c, sft);
+    }
+    if (lane == 31) s_tot[0][tid >> 5] = xa;
+    if (lane == 0) {
+        s_tot[1][tid >> 5] = b;
+        s_tot[2][tid >> 5] = c;
+    }
+    __syncthreads();
+    {
+        unsigned long long base = xa - a;
+        for (int k = 0; k < (tid >> 5); ++k) base += s_tot[0][k];
+        for (int i = i0; i < i1; ++i) {
+            ws.tile_base[i] = base;
+            base += *(const volatile unsigned long long*)&ws.tiles[i];
+        }
+    }
+    if (tid < 3) {
+        unsigned long long v = 0;
+        for (int k = 0; k < n_warps; ++k) v += s_tot[tid][k];
+        totals[tid == 2 ? 3 : tid] = (int64_t)v;
+        if (totals_host) totals_host[tid == 2 ? 3 : tid] = (int64_t)v;
+    }
+    if (tid == 3) {
+        totals[2] = ws.run_capacity;
+        if (totals_host) totals_host[2] = ws.run_capacity;
+    }
+    // (no system-scope fence: the host reads the pinned totals after it has waited for this kernel)
+    if (tid == 0) {
+        *ws.done = 0u;
+        *ws.cursor = 0u;
+    }
+}
+
 template <bool kSingle, int kSlots>
 __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p)
 {
     extern __shared__ __align__(16) uint32_t s_dyn[];
     __shared__ __align__(8) uint64_t s_bar;
-    __shared__ unsigned long long s_red_samples[kMaxTileRays / 32];
-    __shared__ uint32_t s_red_runs[kMaxTileRays / 32], s_red_flags[kMaxTileRays / 32], s_wsum[kMaxTileRays / 32];
-    __shared__ bool s_last;
     __shared__ uint32_t s_hist[kSortBuckets];
 
     const int T = blockDim.x;            // threads = rays of a (full) tile
@@ -567,57 +698,9 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
     if (p.trace) {
         tr_c2 = clock64();  // this warp's rays done
     }
-    // ---- tile sums, and grand totals by the last CTA to finish ------------
-    const int n_warps = T >> 5;
-    unsigned long long vs = active ? m.n_samples : 0u;
-    uint32_t vr = active ? m.n_runs : 0u, vf = (active && !m.ok) ? 1u : 0u;
-#pragma unroll
-    for (int sft = 16; sft > 0; sft >>= 1) {
-        vs += __shfl_xor_sync(0xffffffffu, vs, sft);
-        vr += __shfl_xor_sync(0xffffffffu, vr, sft);
-        vf += __shfl_xor_sync(0xffffffffu, vf, sft);
-    }
-    if (lane == 0) {
-        s_red_samples[tid >> 5] = vs;
-        s_red_runs[tid >> 5] = vr;
-        s_red_flags[tid >> 5] = vf;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        TileSum ts;
-        ts.samples = 0;
-        ts.runs = 0;
-        ts.stuck = 0;
-        for (int k = 0; k < n_warps; ++k) {
-            ts.samples += s_red_samples[k];
-            ts.runs += s_red_runs[k];
-            ts.stuck += s_red_flags[k];
-        }
-        p.ws.tiles[tile] = ts;
-        __threadfence();
-        const uint32_t prev = atomicAdd(p.ws.done, 1u);
-        s_last = (prev == (uint32_t)(gridDim.x - 1));
-    }
-    // Samples of the earlier rays of this tile, in RAY order (the threads hold the rays in sorted order): with the
-    // tile bases below this is every ray's packed_info start, so that no separate offsets pass has to run before the
-    // samples are expanded.  The descriptor buffers are free by now (barrier above): counts go through them.
-    uint32_t* s_cnt = reinterpret_cast<uint32_t*>(s_pend);
-    if (active) s_cnt[rt] = m.n_samples;
-    __syncthreads();
-    {
-        const uint32_t cs = tid < nr ? s_cnt[tid] : 0u;
-        uint32_t xs = cs;
-#pragma unroll
-        for (int sft = 1; sft < 32; sft <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xffffffffu, xs, sft);
-            if (lane >= sft) xs += y;
-        }
-        if (lane == 31) s_wsum[tid >> 5] = xs;
-        __syncthreads();
-        uint32_t before = xs - cs;
-        for (int k = 0; k < (tid >> 5); ++k) before += s_wsum[k];
-        if (tid < nr) p.ws.loc_samples[r0 + tid] = before;
-    }
+    // the descriptor buffers are free by now: the tile's counts go through them
+    const bool last = march_tile_sums(p.ws, r0, nr, rt, active, m.n_samples, m.n_runs, !m.ok,
+                                      reinterpret_cast<uint32_t*>(s_pend));
     if (p.trace && lane == 0) {
         tr_c3 = clock64();  // past the tile's last barrier
         unsigned long long t1;
@@ -628,63 +711,7 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
         q[0] = tr_t0; q[1] = t1; q[2] = tr_c1 - tr_c0; q[3] = tr_c2 - tr_c0; q[4] = tr_c3 - tr_c0; q[5] = smid;
         q[6] = ((unsigned long long)tr_loops << 48) | ((tr_w - tr_c0) & 0xffffffffffffull); q[7] = 1;
     }
-    if (s_last) {
-        __threadfence();
-        // tile bases (exclusive scan of the tile sums: a contiguous chunk of tiles per thread) and the grand totals
-        const int n_tiles = p.ws.n_tiles;
-        const int chunk = (n_tiles + T - 1) / T;
-        const int i0 = min(tid * chunk, n_tiles), i1 = min(i0 + chunk, n_tiles);
-        unsigned long long a = 0, b = 0, c = 0;
-        for (int i = i0; i < i1; ++i) {
-            const volatile unsigned long long* q = (const volatile unsigned long long*)&p.ws.tiles[i];
-            const unsigned long long w0 = q[0], w1 = q[1];  // {samples}, {runs | stuck << 32}
-            a += w0;
-            b += (uint32_t)w1;
-            c += w1 >> 32;
-        }
-        unsigned long long xa = a;
-#pragma unroll
-        for (int sft = 1; sft < 32; sft <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, xa, sft);
-            if (lane >= sft) xa += y;
-        }
-#pragma unroll
-        for (int sft = 16; sft > 0; sft >>= 1) {
-            b += __shfl_xor_sync(0xffffffffu, b, sft);
-            c += __shfl_xor_sync(0xffffffffu, c, sft);
-        }
-        __shared__ unsigned long long s_tot[3][kMaxTileRays / 32];
-        if (lane == 31) s_tot[0][tid >> 5] = xa;
-        if (lane == 0) {
-            s_tot[1][tid >> 5] = b;
-            s_tot[2][tid >> 5] = c;
-        }
-        __syncthreads();
-        {
-            unsigned long long base = xa - a;
-            for (int k = 0; k < (tid >> 5); ++k) base += s_tot[0][k];
-            for (int i = i0; i < i1; ++i) {
-                p.ws.tile_base[i] = base;
-                base += *(const volatile unsigned long long*)&p.ws.tiles[i];
-            }
-        }
-        if (tid < 3) {
-            unsigned long long v = 0;
-            for (int k = 0; k < n_warps; ++k) v += s_tot[tid][k];
-            // totals: [0] samples, [1] runs, [2] run-pool capacity used for this call, [3] stuck rays
-            p.totals[tid == 2 ? 3 : tid] = (int64_t)v;
-            if (p.totals_host) p.totals_host[tid == 2 ? 3 : tid] = (int64_t)v;
-        }
-        if (tid == 3) {
-            p.totals[2] = p.ws.run_capacity;
-            if (p.totals_host) p.totals_host[2] = p.ws.run_capacity;
-        }
-        // (no system-scope fence: the host reads the pinned totals after it has waited for this kernel)
-        if (tid == 0) {  // leave the workspace reusable
-            *p.ws.done = 0u;
-            *p.ws.cursor = 0u;
-        }
-    }
+    if (last) march_totals(p.ws, p.totals, p.totals_host);
 }
 
 // ---------------------------------------------------------------------------
@@ -857,6 +884,19 @@ __global__ void __launch_bounds__(kExpandThreads) expand_runs_kernel(const Expan
     }
 }
 
+// packed_info of every ray = [base of the ray's march tile + samples of the tile's earlier rays, count]: the march
+// kernel left both parts in the workspace, so no offsets pass runs in front of the samples-only expand kernels.  Their
+// runs take their offsets from the same two arrays, not from packed_info (another CTA may not have written it yet).
+__device__ __forceinline__ void write_packed_info(const Workspace& ws, int32_t n_rays, int64_t* packed_out)
+{
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n_rays; r += (int64_t)gridDim.x * blockDim.x) {
+        longlong2 v;
+        v.x = (long long)(ws.tile_base[r / ws.tile_rays] + ws.loc_samples[r]);
+        v.y = (long long)ws.cnt_samples[r];
+        *reinterpret_cast<longlong2*>(packed_out + 2 * r) = v;
+    }
+}
+
 // Samples-only expansion with 128-bit stores: a piece (lattice.cuh) of a run is written as an
 // unaligned head (< 4 samples), a body of output groups [4G, 4G+3] -- one lane per group: a float4 of
 // starts, a float4 of ends, two longlong2 of ray ids -- and a tail.  Same values as the scalar kernel.
@@ -870,16 +910,7 @@ __global__ void __launch_bounds__(kExpandThreads) expand_runs_vec_kernel(const E
     int64_t n_runs = p.totals[1];
     if (n_runs > p.ws.run_capacity) n_runs = p.ws.run_capacity;
     const Lattice L = lat_make(p.step_size);
-    // packed_info of every ray = [base of the ray's march tile + samples of the tile's earlier rays, count]: the march
-    // kernel left both parts in the workspace, so no offsets pass runs in front of this kernel.  The runs below take
-    // their offsets from the same two arrays, not from packed_info (another CTA may not have written it yet).
-    for (int64_t r = (int64_t)blockIdx.x * kExpandThreads + threadIdx.x; r < p.n_rays;
-         r += (int64_t)gridDim.x * kExpandThreads) {
-        longlong2 v;
-        v.x = (long long)(p.ws.tile_base[r / p.ws.tile_rays] + p.ws.loc_samples[r]);
-        v.y = (long long)p.ws.cnt_samples[r];
-        *reinterpret_cast<longlong2*>(p.packed_out + 2 * r) = v;
-    }
+    write_packed_info(p.ws, p.n_rays, p.packed_out);
     for (int64_t q = warp0; q < n_runs; q += n_warps) {
         const uint4 a = __ldg(reinterpret_cast<const uint4*>(p.ws.pool + q));
         const uint32_t run_tile = __ldg(&p.ws.pool[q].tile);
@@ -1001,6 +1032,146 @@ __global__ void __launch_bounds__(128) generic_traverse_kernel(const GenericPara
     if (p.terminate) p.terminate[r] = term;
     p.iv_cnts[r] = out.n_edges;
     p.sm_cnts[r] = out.n_samples;
+}
+
+// ---------------------------------------------------------------------------
+// growing steps (cone_angle > 0): walk -> runs -> expand, the layout of the constant-step path
+// ---------------------------------------------------------------------------
+struct ConeParams {
+    int32_t n_rays;
+    const float* rays_o;
+    const float* rays_d;
+    const float* near_planes;  // per ray, or null: near_plane for every ray
+    const float* far_planes;
+    float near_plane, far_plane;
+    OccGeom g;
+    const uint64_t* words;
+    const uint32_t* coarse;
+    const float* aabbs;
+    const float* t_sorted;  // null: one level, crossings computed in the kernel
+    const int64_t* t_indices;
+    const uint8_t* hits;
+    float step_size, cone_angle;
+    Workspace ws;
+    int64_t* totals;
+    int64_t* totals_host;
+};
+
+// RunSink pool of the march kernel: the lanes that close a run at the same time take their slots with one atomic
+struct PoolAppend {
+    uint32_t* cursor;
+    RunRec* pool;
+    int64_t capacity;
+    uint32_t ray, tile;
+    __device__ __forceinline__ void put(uint32_t sample_off, uint32_t n, float t_first, uint32_t run_idx)
+    {
+        const cg::coalesced_group g = cg::coalesced_threads();
+        uint32_t base = 0;
+        if (g.thread_rank() == 0) base = atomicAdd(cursor, (uint32_t)g.size());
+        const uint32_t slot = g.shfl(base, 0) + (uint32_t)g.thread_rank();
+        if ((int64_t)slot < capacity) {
+            uint4* dst = reinterpret_cast<uint4*>(pool + slot);
+            dst[0] = make_uint4(ray, sample_off, n, __float_as_uint(t_first));
+            dst[1] = make_uint4(run_idx, tile, 0u, 0u);
+        }
+    }
+};
+
+// One thread per ray, tiles of ws.tile_rays rays in ray order, the walk of march_generic.cuh.  A ray whose marching
+// variable stops advancing ends there, as in generic_traverse_kernel: the stuck count stays 0.
+template <bool kSingle>
+__global__ void __launch_bounds__(kMaxTileRays) march_cone_kernel(const ConeParams p)
+{
+    __shared__ uint32_t s_cnt[kMaxTileRays];
+    const int tid = threadIdx.x;
+    const int r0 = blockIdx.x * blockDim.x;
+    const int nr = min((int)blockDim.x, p.n_rays - r0);
+    const int r = r0 + tid;
+    const bool active = tid < nr;
+    RunSink<PoolAppend> out;
+    run_sink_init(out);
+    out.pool.cursor = p.ws.cursor;
+    out.pool.pool = p.ws.pool;
+    out.pool.capacity = p.ws.run_capacity;
+    out.pool.ray = (uint32_t)r;
+    out.pool.tile = blockIdx.x;
+    if (active) {
+        OccView occ;
+        occ.words = p.words;
+        occ.coarse = p.coarse;
+        occ.bounds = nullptr;
+        occ.g = p.g;
+        const float o[3] = {p.rays_o[3 * (int64_t)r], p.rays_o[3 * (int64_t)r + 1], p.rays_o[3 * (int64_t)r + 2]};
+        const float d[3] = {p.rays_d[3 * (int64_t)r], p.rays_d[3 * (int64_t)r + 1], p.rays_d[3 * (int64_t)r + 2]};
+        const float near = p.near_planes ? p.near_planes[r] : p.near_plane;
+        const float far = p.far_planes ? p.far_planes[r] : p.far_plane;
+        if (kSingle) {
+            const SingleBox boxes{p.aabbs};
+            generic_march_ray(boxes, occ, o, d, near, far, p.step_size, p.cone_angle, -1, out);
+        } else {
+            const int G = p.g.n_grids;
+            const SortedBoxes boxes{p.aabbs, G, p.t_sorted + (int64_t)r * 2 * G, p.t_indices + (int64_t)r * 2 * G,
+                                    p.hits + (int64_t)r * G};
+            generic_march_ray(boxes, occ, o, d, near, far, p.step_size, p.cone_angle, -1, out);
+        }
+        run_sink_close(out);
+        p.ws.cnt_samples[r] = (uint32_t)out.n_samples;
+        p.ws.cnt_runs[r] = out.n_runs;
+    }
+    if (march_tile_sums(p.ws, r0, nr, tid, active, (uint32_t)out.n_samples, out.n_runs, false, s_cnt))
+        march_totals(p.ws, p.totals, p.totals_host);
+}
+
+// packed_info, then the runs, 32 per warp and round: each lane loads one run record and its output offset
+// [tile base + samples of the tile's earlier rays + samples of the ray before the run] (the dependent loads of 32
+// runs in flight together), then the warp writes the runs one after the other, lane j sample j of each piece of 32
+// (march_generic.cuh, cone_expand_run: the same float operations in the same order), so that stores coalesce.
+__global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const Workspace ws, int32_t n_rays,
+                                                                     const int64_t* totals, float step_size,
+                                                                     float cone_angle, int64_t capacity,
+                                                                     int64_t* packed_info, int64_t* ray_indices,
+                                                                     float* t_starts, float* t_ends)
+{
+    static_assert(kExpandLanes == 32, "one lane per sample of a piece");
+    write_packed_info(ws, n_rays, packed_info);
+    int64_t n_runs = totals[1];
+    if (n_runs > ws.run_capacity) n_runs = ws.run_capacity;  // the host re-runs with a larger pool
+    const int lane = threadIdx.x & 31;
+    const int64_t warp0 = ((int64_t)blockIdx.x * kExpandThreads + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * kExpandThreads) >> 5;
+    for (int64_t q0 = warp0 * 32; q0 < n_runs; q0 += n_warps * 32) {
+        const int64_t q = q0 + lane;
+        uint32_t my_n = 0, my_ray = 0;
+        float my_first = 0.f;
+        int64_t my_k0 = 0;
+        if (q < n_runs) {
+            const uint4 a = __ldg(reinterpret_cast<const uint4*>(ws.pool + q));
+            const uint32_t tile = __ldg(&ws.pool[q].tile);
+            my_ray = a.x;
+            my_n = a.z;
+            my_first = __uint_as_float(a.w);
+            my_k0 = (int64_t)(ws.tile_base[tile] + ws.loc_samples[a.x]) + a.y;
+        }
+        for (int i = 0; i < 32; ++i) {
+            const uint32_t n = __shfl_sync(0xffffffffu, my_n, i);
+            if (n == 0u) continue;  // past the last run
+            const long long ray = (long long)__shfl_sync(0xffffffffu, my_ray, i);
+            const int64_t k0 = __shfl_sync(0xffffffffu, my_k0, i);
+            float t = __shfl_sync(0xffffffffu, my_first, i);
+            for (uint32_t base = 0; base < n; base += 32) {
+                const uint32_t m = min(n - base, 32u);
+                const float ts = cone_advance(t, min((uint32_t)lane, m - 1u), cone_angle, step_size);
+                const float te = cone_next(ts, cone_angle, step_size);
+                const int64_t k = k0 + base + lane;
+                if ((uint32_t)lane < m && k < capacity) {
+                    ray_indices[k] = ray;
+                    t_starts[k] = ts;
+                    t_ends[k] = te;
+                }
+                t = __shfl_sync(0xffffffffu, te, (int)m - 1);
+            }
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------
@@ -1319,6 +1490,72 @@ int32_t nfa_expand_intervals(int32_t n_rays, int64_t run_capacity, const void* w
         p.sm_is_valid = sm_is_valid;
         expand_runs_kernel<true><<<expand_grid(run_capacity), kExpandThreads, 0, s>>>(p);
     }
+    return launch_status();
+}
+
+int32_t nfa_march_cone(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
+                       const float* far_planes, float near_plane, float far_plane, int32_t n_grids, int32_t rx,
+                       int32_t ry, int32_t rz, const uint64_t* words, const uint32_t* coarse, const float* aabbs,
+                       const float* t_sorted, const int64_t* t_indices, const uint8_t* hits, float step_size,
+                       float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
+                       int64_t* totals_host, nfa_stream_t stream)
+{
+    if (n_rays < 0 || n_grids <= 0 || rx <= 0 || ry <= 0 || rz <= 0 || run_capacity < 0) return NFA_ERR_ARG;
+    if (run_capacity > (int64_t)UINT32_MAX) return NFA_ERR_UNSUPPORTED;
+    if (!(step_size > 0.0f)) return NFA_ERR_UNSUPPORTED;
+    if (!totals) return NFA_ERR_ARG;
+    if ((near_planes == nullptr) != (far_planes == nullptr)) return NFA_ERR_ARG;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n_rays == 0) {
+        if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
+        return (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
+    }
+    if (!rays_o || !rays_d || !words || !coarse || !aabbs || !workspace) return NFA_ERR_ARG;
+    const bool have_sorted = t_sorted && t_indices && hits;
+    if (!have_sorted && n_grids != 1) return NFA_ERR_ARG;
+    ConeParams p;
+    p.n_rays = n_rays;
+    p.rays_o = rays_o;
+    p.rays_d = rays_d;
+    p.near_planes = near_planes;
+    p.far_planes = far_planes;
+    p.near_plane = near_plane;
+    p.far_plane = far_plane;
+    p.g = occ_geom(n_grids, rx, ry, rz);
+    p.words = words;
+    p.coarse = coarse;
+    p.aabbs = aabbs;
+    p.t_sorted = have_sorted ? t_sorted : nullptr;
+    p.t_indices = have_sorted ? t_indices : nullptr;
+    p.hits = have_sorted ? hits : nullptr;
+    p.step_size = step_size;
+    p.cone_angle = cone_angle;
+    p.ws = ws_view(workspace, n_rays, run_capacity);
+    p.totals = totals;
+    p.totals_host = totals_host;
+    if (have_sorted) march_cone_kernel<false><<<p.ws.n_tiles, p.ws.tile_rays, 0, s>>>(p);
+    else march_cone_kernel<true><<<p.ws.n_tiles, p.ws.tile_rays, 0, s>>>(p);
+    return launch_status();
+}
+
+int32_t nfa_expand_cone_samples(int32_t n_rays, int64_t run_capacity, const void* workspace, const int64_t* totals,
+                                float step_size, float cone_angle, int64_t capacity, int64_t* packed_info,
+                                int64_t* ray_indices, float* t_starts, float* t_ends, nfa_stream_t stream)
+{
+    if (n_rays < 0 || capacity < 0 || run_capacity < 0) return NFA_ERR_ARG;
+    if (n_rays == 0) return NFA_OK;
+    if (!workspace || !packed_info || !totals) return NFA_ERR_ARG;
+    if (capacity > 0 && (!ray_indices || !t_starts || !t_ends)) return NFA_ERR_ARG;
+    if ((((uintptr_t)packed_info) & 15u) != 0) return NFA_ERR_ARG;
+    const Workspace ws = ws_view(const_cast<void*>(workspace), n_rays, run_capacity);
+    // enough threads for the packed_info prologue and for every run of the pool
+    const int64_t work = run_capacity > n_rays ? run_capacity : n_rays;
+    const int64_t ctas = (work + kExpandThreads - 1) / kExpandThreads;
+    const int64_t cap = kNumSMs * 8;
+    const int grid = (int)(ctas < 1 ? 1 : (ctas < cap ? ctas : cap));
+    expand_cone_kernel<<<grid, kExpandThreads, 0, (cudaStream_t)stream>>>(ws, n_rays, totals, step_size, cone_angle,
+                                                                          capacity, packed_info, ray_indices, t_starts,
+                                                                          t_ends);
     return launch_status();
 }
 

@@ -100,10 +100,11 @@ class OccGridEstimator(AbstractEstimator):
         (transmittance < early_stop_eps) or transparent (alpha < alpha_thre) are dropped.
         Not differentiable.  Semantics: reference occ_grid.py:85-221.
         """
-        fast = cone_angle == 0.0 and render_step_size > 0.0 and rays_o.is_cuda
+        fast = cone_angle >= 0.0 and render_step_size > 0.0 and rays_o.is_cuda
         if fast:
             ticket = self.sampling_begin(rays_o, rays_d, near_plane=near_plane, far_plane=far_plane, t_min=t_min,
-                                         t_max=t_max, render_step_size=render_step_size, stratified=stratified)
+                                         t_max=t_max, render_step_size=render_step_size, stratified=stratified,
+                                         cone_angle=cone_angle)
             return self.sampling_end(ticket, sigma_fn=sigma_fn, alpha_fn=alpha_fn, early_stop_eps=early_stop_eps,
                                      alpha_thre=alpha_thre)
         near_planes, far_planes = self._ray_planes(rays_o, near_plane, far_plane, t_min, t_max, stratified,
@@ -127,24 +128,29 @@ class OccGridEstimator(AbstractEstimator):
         t_max: Optional[Tensor] = None,
         render_step_size: float = 1e-3,
         stratified: bool = False,
+        cone_angle: float = 0.0,
     ):
-        """First half of :meth:`sampling` (constant step, CUDA): queue the traversal and return a ticket at once.
+        """First half of :meth:`sampling` (CUDA, render_step_size > 0, cone_angle >= 0): queue the traversal and
+        return a ticket at once.
 
         The size of a batch is only known once the traversal has run, so ``sampling()`` has to wait for the GPU
         once per call -- on a training step that is host-bound that wait (and the kernel itself) sits on the
         critical path.  A loop that knows its next rays early can call ``sampling_begin`` for batch k+1 before
         ``loss.backward()`` of batch k and ``sampling_end`` at the top of step k+1: the traversal then runs behind
         the backward kernels while the host is busy, and ``sampling_end`` returns without waiting.  The occupancy
-        grid is read when the traversal runs; call ``sampling_end`` before changing it.  Not part of nerfacc's API.
+        grid is read when the traversal runs; call ``sampling_end`` before changing it.  With ``cone_angle > 0``
+        (unbounded scenes: the step grows with the distance) the same split applies.  Not part of nerfacc's API.
         """
-        if not (rays_o.is_cuda and render_step_size > 0.0):
-            raise ValueError("sampling_begin: only the constant-step CUDA path can be split; use sampling().")
+        if not (rays_o.is_cuda and render_step_size > 0.0 and cone_angle >= 0.0):
+            raise ValueError("sampling_begin: only CUDA rays with render_step_size > 0 and cone_angle >= 0 can be "
+                             "split; use sampling().")
         near_planes, far_planes = self._ray_planes(rays_o, near_plane, far_plane, t_min, t_max, stratified,
                                                    render_step_size, always=False)
         return _MarchJob(rays_o.contiguous().float(), rays_d.contiguous().float(), self.binaries,
                          self.aabbs.contiguous().float(), near_planes, far_planes, float(render_step_size), None, None,
                          None, want_intervals=False, want_terminate=False, capacity_hint=self._capacity_hint,
-                         near_plane=float(near_plane), far_plane=float(far_plane)).begin()
+                         near_plane=float(near_plane), far_plane=float(far_plane),
+                         cone_angle=float(cone_angle)).begin()
 
     @torch.no_grad()
     def sampling_end(

@@ -172,18 +172,25 @@ class _MarchResult:
 
 
 class _MarchJob:
-    """Constant-step traversal: march -> expand, with ONE host synchronisation, in two halves.
+    """Traversal by runs: march -> expand, with ONE host synchronisation, in two halves.
 
     `begin()` queues the march and, given a `capacity_hint` (size of the previous batch plus head-room), the
     expand kernels behind it; `finish()` waits for the totals, re-runs the cheap tail only if the batch outgrew
     the hint (or the run pool) and returns the result.  `near_planes` / `far_planes` may both be None: every ray
     then uses the scalars.  The job keeps its inputs alive and owns its workspace until `finish()`.
+
+    `cone_angle == 0`: constant step (nfa_march / nfa_expand_*).  `cone_angle > 0`: the step grows with the distance
+    (nfa_march_cone / nfa_expand_cone_samples), samples only -- no interval form, no terminate planes.
     """
 
     def __init__(self, rays_o: Tensor, rays_d: Tensor, binaries: Tensor, aabbs: Tensor, near_planes: Optional[Tensor],
                  far_planes: Optional[Tensor], step_size: float, t_sorted: Optional[Tensor],
                  t_indices: Optional[Tensor], hits: Optional[Tensor], want_intervals: bool, want_terminate: bool,
-                 capacity_hint: int = 0, near_plane: float = 0.0, far_plane: float = float("inf")):
+                 capacity_hint: int = 0, near_plane: float = 0.0, far_plane: float = float("inf"),
+                 cone_angle: float = 0.0):
+        self.cone_angle = float(cone_angle)
+        if self.cone_angle != 0.0:
+            assert self.cone_angle > 0.0 and not want_intervals and not want_terminate
         self.device = device = rays_o.device
         self.n_rays = n_rays = rays_o.shape[0]
         self.shape = tuple(int(s) for s in binaries.shape)
@@ -214,11 +221,18 @@ class _MarchJob:
         rays_o, rays_d, aabbs, near_planes, far_planes, t_sorted, t_indices, hits = self.inputs
         n_grids, rx, ry, rz = self.shape
         sc, occ = self.sc, self.occ
-        _lib.call("nfa_march", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(near_planes),
-                  _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz, _lib.ptr(occ.words),
-                  _lib.ptr(occ.bounds), _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices),
-                  _lib.ptr(hits), self.step_size, sc.run_capacity, _lib.ptr(sc.workspace), _lib.ptr(sc.totals_dev),
-                  _lib.ptr(sc.totals_host), _lib.ptr(self.term))
+        if self.cone_angle > 0.0:
+            _lib.call("nfa_march_cone", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d),
+                      _lib.ptr(near_planes), _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz,
+                      _lib.ptr(occ.words), _lib.ptr(occ.coarse), _lib.ptr(aabbs), _lib.ptr(t_sorted),
+                      _lib.ptr(t_indices), _lib.ptr(hits), self.step_size, self.cone_angle, sc.run_capacity,
+                      _lib.ptr(sc.workspace), _lib.ptr(sc.totals_dev), _lib.ptr(sc.totals_host))
+        else:
+            _lib.call("nfa_march", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(near_planes),
+                      _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz, _lib.ptr(occ.words),
+                      _lib.ptr(occ.bounds), _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices),
+                      _lib.ptr(hits), self.step_size, sc.run_capacity, _lib.ptr(sc.workspace), _lib.ptr(sc.totals_dev),
+                      _lib.ptr(sc.totals_host), _lib.ptr(self.term))
         # on the stream (of THIS device) the march was launched on: the default `record()` would use the current
         # device's stream and the totals could be read before they are written
         sc.event.record(torch.cuda.current_stream(self.device))
@@ -242,9 +256,14 @@ class _MarchJob:
         ri = torch.empty(cap, dtype=torch.int64, device=device)
         ts = torch.empty(cap, dtype=torch.float32, device=device)
         te = torch.empty(cap, dtype=torch.float32, device=device)
-        _lib.call("nfa_expand_samples", device, self.n_rays, sc.run_capacity, _lib.ptr(sc.workspace),
-                  _lib.ptr(sc.totals_dev), self.step_size, cap, _lib.ptr(self.packed_info), _lib.ptr(ri), _lib.ptr(ts),
-                  _lib.ptr(te))
+        if self.cone_angle > 0.0:
+            _lib.call("nfa_expand_cone_samples", device, self.n_rays, sc.run_capacity, _lib.ptr(sc.workspace),
+                      _lib.ptr(sc.totals_dev), self.step_size, self.cone_angle, cap, _lib.ptr(self.packed_info),
+                      _lib.ptr(ri), _lib.ptr(ts), _lib.ptr(te))
+        else:
+            _lib.call("nfa_expand_samples", device, self.n_rays, sc.run_capacity, _lib.ptr(sc.workspace),
+                      _lib.ptr(sc.totals_dev), self.step_size, cap, _lib.ptr(self.packed_info), _lib.ptr(ri),
+                      _lib.ptr(ts), _lib.ptr(te))
         return ri, ts, te
 
     def begin(self) -> "_MarchJob":

@@ -130,8 +130,8 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d,
  *   replaces the fill pass plus `vals[is_left]`, `vals[is_right]` of
  *   nerfacc/estimators/occ_grid.py:174-177.  `totals` is the device array nfa_march
  *   filled.  Elements at index >= capacity are not written (the caller re-runs with a
- *   larger buffer).  packed_info: [n_rays, 2] = (chunk_start, chunk_cnt), written by this call
- *   (inside the expand kernel when the outputs are 16-byte aligned: one launch). */
+ *   larger buffer).  packed_info: [n_rays, 2] = (chunk_start, chunk_cnt), always written by this call
+ *   (in the one kernel it launches, also when capacity or run_capacity is 0). */
 int32_t nfa_expand_samples(int32_t n_rays, int64_t run_capacity, const void* workspace,
                            const int64_t* totals, float step_size, int64_t capacity,
                            int64_t* packed_info, int64_t* ray_indices, float* t_starts, float* t_ends,

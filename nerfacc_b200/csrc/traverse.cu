@@ -13,14 +13,14 @@
 //                     lattice seeks, a warp's stretches dealt out to its lanes (march.cuh).  Runs go to a pool
 //                     (one atomic per warp and round); per-ray counts, each ray's sample offset inside its tile,
 //                     per-tile sums and (last CTA) the tile bases + grand totals are left in the workspace.
-//   offsets_kernel    1 CTA / tile: tile base from the tile sums + block scan -> packed_info (ray-ordered
-//                     offsets, so ray_indices stay sorted).  Interval form and the scalar fallback only: the
-//                     vectorised samples kernel writes packed_info itself from (tile base, offset in tile).
-//   expand_runs_vec_kernel / expand_runs_kernel
-//                     one warp per run: lanes compute their samples from the lattice
-//                     closed form (expand.cuh) and store them coalesced, 128-bit stores
-//                     when the outputs are 16-byte aligned; the <true> flavour writes the
-//                     interval-edge form traverse_grids() returns.
+//   expand_samples_kernel
+//                     packed_info from (tile base, offset in tile), then one warp per run: lanes compute their
+//                     samples from the lattice closed form (expand.cuh) and store them coalesced, 128-bit stores
+//                     when the outputs are 16-byte aligned (<true>), element-wise otherwise (<false>).
+//   offsets_kernel / expand_intervals_kernel
+//                     the interval-edge form traverse_grids() returns: 1 CTA / tile scans the tile sums and the
+//                     per-ray sample and run counts into both packed_infos (ray-ordered offsets, so ray_indices
+//                     stay sorted), then one warp per run writes the edges and the samples.
 //   march_cone_kernel / expand_cone_kernel
 //                     sampling() with growing steps (cone_angle > 0): 1 thread / ray walks sample by sample
 //                     (march_generic.cuh) into the same run pool, counts and tile sums as march_kernel;
@@ -269,6 +269,18 @@ struct SmemBuf {
     }
 };
 
+// The one writer of a run record: slot `slot` of the pool, dropped when the pool is full (the march still counts the
+// run, and the host re-marches with a larger pool).
+__device__ __forceinline__ void store_run(RunRec* pool, int64_t capacity, uint32_t slot, uint32_t ray, uint32_t tile,
+                                          uint32_t sample_off, uint32_t n, float t_first, uint32_t run_idx)
+{
+    if ((int64_t)slot < capacity) {
+        uint4* dst = reinterpret_cast<uint4*>(pool + slot);
+        dst[0] = make_uint4(ray, sample_off, n, __float_as_uint(t_first));
+        dst[1] = make_uint4(run_idx, tile, 0u, 0u);
+    }
+}
+
 // append the runs the lanes of a warp closed in this step: one atomic per warp
 __device__ __forceinline__ void emit_runs(const RunOut& out, uint32_t ray, uint32_t tile, const Workspace& ws, int lane)
 {
@@ -278,14 +290,9 @@ __device__ __forceinline__ void emit_runs(const RunOut& out, uint32_t ray, uint3
     uint32_t base = 0;
     if (lane == leader) base = atomicAdd(ws.cursor, (uint32_t)__popc(mask));
     base = __shfl_sync(0xffffffffu, base, leader);
-    if (out.valid) {
-        const uint32_t slot = base + (uint32_t)__popc(mask & ((1u << lane) - 1u));
-        if ((int64_t)slot < ws.run_capacity) {
-            uint4* dst = reinterpret_cast<uint4*>(ws.pool + slot);
-            dst[0] = make_uint4(ray, out.sample_off, out.n, __float_as_uint(out.t_first));
-            dst[1] = make_uint4(out.run_idx, tile, 0u, 0u);
-        }
-    }
+    if (out.valid)
+        store_run(ws.pool, ws.run_capacity, base + (uint32_t)__popc(mask & ((1u << lane) - 1u)), ray, tile,
+                  out.sample_off, out.n, out.t_first, out.run_idx);
 }
 
 // dynamic shared memory of the march kernel (tile = blockDim.x rays):
@@ -654,11 +661,8 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
                     RunOut out;
                     lat_take(m, s_pend[j * T + tid], __float_as_uint(s_open[j * T + tid]), out);
                     if (out.valid) {
-                        if ((int64_t)slot < p.ws.run_capacity) {
-                            uint4* dst = reinterpret_cast<uint4*>(p.ws.pool + slot);
-                            dst[0] = make_uint4((uint32_t)r, out.sample_off, out.n, __float_as_uint(out.t_first));
-                            dst[1] = make_uint4(out.run_idx, (uint32_t)tile, 0u, 0u);
-                        }
+                        store_run(p.ws.pool, p.ws.run_capacity, slot, (uint32_t)r, (uint32_t)tile, out.sample_off,
+                                  out.n, out.t_first, out.run_idx);
                         ++slot;
                     }
                 }
@@ -715,9 +719,9 @@ __global__ void __launch_bounds__(kMaxTileRays) march_kernel(const MarchParams p
 }
 
 // ---------------------------------------------------------------------------
-// offsets: per-ray packed_info from the counts (tile base from the tile sums + block scan)
+// offsets of the interval form: both per-ray packed_infos from the counts (tile base from the tile sums + block
+// scan).  The edges of a ray start after the runs of the earlier rays, which the march does not scan.
 // ---------------------------------------------------------------------------
-template <bool kIntervals>
 __global__ void __launch_bounds__(kMaxTileRays) offsets_kernel(int32_t n_rays, Workspace ws, int64_t* sm_packed_info,
                                                               int64_t* iv_packed_info)
 {
@@ -787,58 +791,162 @@ __global__ void __launch_bounds__(kMaxTileRays) offsets_kernel(int32_t n_rays, W
         v.x = (long long)off;
         v.y = (long long)cs;
         *reinterpret_cast<longlong2*>(sm_packed_info + 2 * (int64_t)(r0 + tid)) = v;
-        if (kIntervals) {
-            longlong2 e;  // a run of n samples has n + 1 edges
-            e.x = (long long)(off + s_base[1] + wrun + (xr - cr));
-            e.y = (long long)cs + (long long)cr;
-            *reinterpret_cast<longlong2*>(iv_packed_info + 2 * (int64_t)(r0 + tid)) = e;
-        }
+        longlong2 e;  // a run of n samples has n + 1 edges
+        e.x = (long long)(off + s_base[1] + wrun + (xr - cr));
+        e.y = (long long)cs + (long long)cr;
+        *reinterpret_cast<longlong2*>(iv_packed_info + 2 * (int64_t)(r0 + tid)) = e;
     }
 }
 
 // ---------------------------------------------------------------------------
 // expand: runs -> per-sample arrays, one warp per run, coalesced stores
 // ---------------------------------------------------------------------------
-struct ExpandParams {
+// Runs in the pool: a march that overflowed it counted more than it stored (the host re-runs with a larger pool).
+__device__ __forceinline__ int64_t pool_runs(const Workspace& ws, const int64_t* totals)
+{
+    int64_t n_runs = totals[1];
+    if (n_runs > ws.run_capacity) n_runs = ws.run_capacity;
+    return n_runs;
+}
+
+// The one reader of a run record for the samples form: its first 16 bytes (ray, sample_off, n, t_first) and, in `k0`,
+// the packed index of its first sample = base of the ray's march tile + samples of the tile's earlier rays +
+// sample_off.  Both parts come from the march, not from packed_info: another CTA may not have written that yet.
+__device__ __forceinline__ uint4 load_run(const Workspace& ws, int64_t q, int64_t& k0)
+{
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(ws.pool + q));
+    const uint32_t tile = __ldg(&ws.pool[q].tile);
+    k0 = (int64_t)(ws.tile_base[tile] + ws.loc_samples[a.x]) + a.y;
+    return a;
+}
+
+// packed_info of every ray = [base of the ray's march tile + samples of the tile's earlier rays, count]: the march
+// kernel left both parts in the workspace, so no offsets pass runs in front of the samples expand kernels.
+__device__ __forceinline__ void write_packed_info(const Workspace& ws, int32_t n_rays, int64_t* packed_out)
+{
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n_rays; r += (int64_t)gridDim.x * blockDim.x) {
+        longlong2 v;
+        v.x = (long long)(ws.tile_base[r / ws.tile_rays] + ws.loc_samples[r]);
+        v.y = (long long)ws.cnt_samples[r];
+        *reinterpret_cast<longlong2*>(packed_out + 2 * r) = v;
+    }
+}
+
+struct SamplesParams {
     Workspace ws;
     int32_t n_rays;
     const int64_t* totals;  // device copy of the march totals ([1] = number of runs)
     float step_size;
-    int64_t sample_capacity;
-    const int64_t* sm_packed_info;
-    int64_t* packed_out;  // samples-only vectorised kernel: packed_info is written here, not read
+    int64_t capacity;
+    int64_t* packed_info;
     int64_t* ray_indices;
     float* t_starts;
     float* t_ends;
-    // interval mode
-    int64_t edge_capacity;
-    const int64_t* iv_packed_info;
-    float* iv_vals;
-    int64_t* iv_ray_indices;
-    uint8_t* iv_is_left;
-    uint8_t* iv_is_right;
-    float* sm_vals;
-    uint8_t* sm_is_valid;
 };
 
-template <bool kIntervals>
-__global__ void __launch_bounds__(kExpandThreads) expand_runs_kernel(const ExpandParams p)
+// Samples form: packed_info, then every run, clipped to the capacity, piece by piece (lattice.cuh).  kVec (outputs
+// 16-byte aligned): a piece is written as an unaligned head (< 4 samples), a body of output groups [4G, 4G+3] -- one
+// lane per group: a float4 of starts, a float4 of ends, two longlong2 of ray ids -- and a tail; otherwise lane j
+// writes samples j, j + 32, ... one by one.  Same values either way.
+// (32-bit sample offsets and one division less per run were measured: no change -- the store stream bounds it.)
+template <bool kVec>
+__global__ void __launch_bounds__(kExpandThreads) expand_samples_kernel(const SamplesParams p)
 {
     const int lane = threadIdx.x & 31;
     const int64_t warp0 = ((int64_t)blockIdx.x * kExpandThreads + threadIdx.x) >> 5;
     const int64_t n_warps = ((int64_t)gridDim.x * kExpandThreads) >> 5;
-    int64_t n_runs = p.totals[1];
-    if (n_runs > p.ws.run_capacity) n_runs = p.ws.run_capacity;  // the host re-runs with a larger pool
+    const int64_t n_runs = pool_runs(p.ws, p.totals);
+    const Lattice L = lat_make(p.step_size);
+    write_packed_info(p.ws, p.n_rays, p.packed_info);
+    for (int64_t q = warp0; q < n_runs; q += n_warps) {
+        int64_t off;
+        const uint4 a = load_run(p.ws, q, off);
+        const long long ray = a.x;
+        RunIter it;
+        it.t = __uint_as_float(a.w);
+        it.left = a.z;
+        if (off >= p.capacity) it.left = 0;
+        else if (off + it.left > p.capacity) it.left = (uint32_t)(p.capacity - off);
+        while (it.left > 0) {
+            LatPiece pc;
+            const int64_t c = (int64_t)run_next_piece(L, it, pc);
+            if (!kVec) {
+                for (uint32_t j = lane; j < c; j += 32) {
+                    const float ts = piece_start(pc, j);
+                    p.ray_indices[off + j] = ray;
+                    p.t_starts[off + j] = ts;
+                    p.t_ends[off + j] = f_add(ts, L.dt);
+                }
+            } else {
+                // head: bring `off` to a multiple of 4 (also covers short pieces entirely)
+                const int head = (int)min((int64_t)((4 - (off & 3)) & 3), c);
+                const int64_t body_groups = (c - head) >> 2;
+                const int tail = (int)(c - head - 4 * body_groups);
+                if (lane < head) {
+                    const float ts = piece_start(pc, (uint32_t)lane);
+                    p.ray_indices[off + lane] = ray;
+                    p.t_starts[off + lane] = ts;
+                    p.t_ends[off + lane] = f_add(ts, L.dt);
+                }
+                const int64_t g0 = (off + head) >> 2;
+                for (int64_t gi = lane; gi < body_groups; gi += 32) {
+                    const uint32_t j = (uint32_t)(head + 4 * gi);
+                    float4 s4, e4;
+                    s4.x = piece_start(pc, j);     e4.x = f_add(s4.x, L.dt);
+                    s4.y = piece_start(pc, j + 1); e4.y = f_add(s4.y, L.dt);
+                    s4.z = piece_start(pc, j + 2); e4.z = f_add(s4.z, L.dt);
+                    s4.w = piece_start(pc, j + 3); e4.w = f_add(s4.w, L.dt);
+                    reinterpret_cast<float4*>(p.t_starts)[g0 + gi] = s4;
+                    reinterpret_cast<float4*>(p.t_ends)[g0 + gi] = e4;
+                    const longlong2 rr = make_longlong2(ray, ray);
+                    reinterpret_cast<longlong2*>(p.ray_indices)[2 * (g0 + gi)] = rr;
+                    reinterpret_cast<longlong2*>(p.ray_indices)[2 * (g0 + gi) + 1] = rr;
+                }
+                if (lane < tail) {
+                    const int64_t k = off + head + 4 * body_groups + lane;
+                    const float ts = piece_start(pc, (uint32_t)(head + 4 * body_groups + lane));
+                    p.ray_indices[k] = ray;
+                    p.t_starts[k] = ts;
+                    p.t_ends[k] = f_add(ts, L.dt);
+                }
+            }
+            off += c;
+        }
+    }
+}
+
+struct IntervalsParams {
+    Workspace ws;
+    const int64_t* totals;
+    float step_size;
+    const int64_t* sm_packed_info;  // samples: packed_info as offsets_kernel wrote it, outputs, capacity
+    int64_t* sm_ray_indices;
+    float* sm_vals;
+    uint8_t* sm_is_valid;
+    int64_t sample_capacity;
+    const int64_t* iv_packed_info;  // edges: the same
+    int64_t* iv_ray_indices;
+    float* iv_vals;
+    uint8_t* iv_is_left;
+    uint8_t* iv_is_right;
+    int64_t edge_capacity;
+};
+
+// Interval form: a run of n samples is n + 1 edges (every sample's left edge, then the run's closing edge) and n
+// samples at the interval midpoints.  Every store is checked against its capacity.
+__global__ void __launch_bounds__(kExpandThreads) expand_intervals_kernel(const IntervalsParams p)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t warp0 = ((int64_t)blockIdx.x * kExpandThreads + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * kExpandThreads) >> 5;
+    const int64_t n_runs = pool_runs(p.ws, p.totals);
     const Lattice L = lat_make(p.step_size);
     for (int64_t q = warp0; q < n_runs; q += n_warps) {
         const uint4 a = __ldg(reinterpret_cast<const uint4*>(p.ws.pool + q));
         const int64_t ray = a.x;
         int64_t off = p.sm_packed_info[2 * ray] + a.y;
-        int64_t eoff = 0;
-        if (kIntervals) {
-            const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.ws.pool + q) + 1);
-            eoff = p.iv_packed_info[2 * ray] + a.y + b.x;
-        }
+        const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.ws.pool + q) + 1);
+        int64_t eoff = p.iv_packed_info[2 * ray] + a.y + b.x;
         RunIter it;
         it.t = __uint_as_float(a.w);
         it.left = a.z;
@@ -850,113 +958,28 @@ __global__ void __launch_bounds__(kExpandThreads) expand_runs_kernel(const Expan
                 const float ts = piece_start(pc, j);
                 const float te = f_add(ts, L.dt);
                 const int64_t k = off + j;
-                if (!kIntervals) {
-                    if (k < p.sample_capacity) {
-                        p.ray_indices[k] = ray;
-                        p.t_starts[k] = ts;
-                        p.t_ends[k] = te;
-                    }
-                } else {
-                    if (k < p.sample_capacity) {
-                        p.ray_indices[k] = ray;                     // samples.ray_indices
-                        p.sm_vals[k] = f_mul(f_add(te, ts), 0.5f);  // reference grid.cu:251
-                        p.sm_is_valid[k] = 1;
-                    }
-                    const int64_t e = eoff + j;
-                    if (e < p.edge_capacity) {  // left edge of sample j (reference grid.cu:219-245)
-                        p.iv_vals[e] = ts;
-                        p.iv_ray_indices[e] = ray;
-                        p.iv_is_left[e] = 1;
-                        p.iv_is_right[e] = (first_piece && j == 0) ? 0 : 1;
-                    }
-                    if (it.left == 0 && j == c - 1 && e + 1 < p.edge_capacity) {  // closing edge of the run
-                        p.iv_vals[e + 1] = te;
-                        p.iv_ray_indices[e + 1] = ray;
-                        p.iv_is_left[e + 1] = 0;
-                        p.iv_is_right[e + 1] = 1;
-                    }
+                if (k < p.sample_capacity) {
+                    p.sm_ray_indices[k] = ray;                  // samples.ray_indices
+                    p.sm_vals[k] = f_mul(f_add(te, ts), 0.5f);  // reference grid.cu:251
+                    p.sm_is_valid[k] = 1;
+                }
+                const int64_t e = eoff + j;
+                if (e < p.edge_capacity) {  // left edge of sample j (reference grid.cu:219-245)
+                    p.iv_vals[e] = ts;
+                    p.iv_ray_indices[e] = ray;
+                    p.iv_is_left[e] = 1;
+                    p.iv_is_right[e] = (first_piece && j == 0) ? 0 : 1;
+                }
+                if (it.left == 0 && j == c - 1 && e + 1 < p.edge_capacity) {  // closing edge of the run
+                    p.iv_vals[e + 1] = te;
+                    p.iv_ray_indices[e + 1] = ray;
+                    p.iv_is_left[e + 1] = 0;
+                    p.iv_is_right[e + 1] = 1;
                 }
             }
             off += c;
             eoff += c;
             first_piece = false;
-        }
-    }
-}
-
-// packed_info of every ray = [base of the ray's march tile + samples of the tile's earlier rays, count]: the march
-// kernel left both parts in the workspace, so no offsets pass runs in front of the samples-only expand kernels.  Their
-// runs take their offsets from the same two arrays, not from packed_info (another CTA may not have written it yet).
-__device__ __forceinline__ void write_packed_info(const Workspace& ws, int32_t n_rays, int64_t* packed_out)
-{
-    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n_rays; r += (int64_t)gridDim.x * blockDim.x) {
-        longlong2 v;
-        v.x = (long long)(ws.tile_base[r / ws.tile_rays] + ws.loc_samples[r]);
-        v.y = (long long)ws.cnt_samples[r];
-        *reinterpret_cast<longlong2*>(packed_out + 2 * r) = v;
-    }
-}
-
-// Samples-only expansion with 128-bit stores: a piece (lattice.cuh) of a run is written as an
-// unaligned head (< 4 samples), a body of output groups [4G, 4G+3] -- one lane per group: a float4 of
-// starts, a float4 of ends, two longlong2 of ray ids -- and a tail.  Same values as the scalar kernel.
-// (32-bit sample offsets and one division less per run were measured: no change -- the store stream bounds it.)
-__global__ void __launch_bounds__(kExpandThreads) expand_runs_vec_kernel(const ExpandParams p)
-{
-    using Idx = int64_t;
-    const int lane = threadIdx.x & 31;
-    const int64_t warp0 = ((int64_t)blockIdx.x * kExpandThreads + threadIdx.x) >> 5;
-    const int64_t n_warps = ((int64_t)gridDim.x * kExpandThreads) >> 5;
-    int64_t n_runs = p.totals[1];
-    if (n_runs > p.ws.run_capacity) n_runs = p.ws.run_capacity;
-    const Lattice L = lat_make(p.step_size);
-    write_packed_info(p.ws, p.n_rays, p.packed_out);
-    for (int64_t q = warp0; q < n_runs; q += n_warps) {
-        const uint4 a = __ldg(reinterpret_cast<const uint4*>(p.ws.pool + q));
-        const uint32_t run_tile = __ldg(&p.ws.pool[q].tile);
-        const long long ray = a.x;
-        const int64_t off64 = (int64_t)(p.ws.tile_base[run_tile] + p.ws.loc_samples[ray]) + a.y;
-        RunIter it;
-        it.t = __uint_as_float(a.w);
-        it.left = a.z;
-        if (off64 >= p.sample_capacity) it.left = 0;
-        else if (off64 + it.left > p.sample_capacity) it.left = (uint32_t)(p.sample_capacity - off64);
-        Idx off = (Idx)off64;
-        while (it.left > 0) {
-            LatPiece pc;
-            const Idx c = (Idx)run_next_piece(L, it, pc);
-            // head: bring `off` to a multiple of 4 (also covers short pieces entirely)
-            const int head = (int)min((Idx)((4 - (off & 3)) & 3), c);
-            const Idx body_groups = (c - head) >> 2;
-            const int tail = (int)(c - head - 4 * body_groups);
-            if (lane < head) {
-                const float ts = piece_start(pc, (uint32_t)lane);
-                p.ray_indices[off + lane] = ray;
-                p.t_starts[off + lane] = ts;
-                p.t_ends[off + lane] = f_add(ts, L.dt);
-            }
-            const Idx g0 = (off + head) >> 2;
-            for (Idx gi = lane; gi < body_groups; gi += 32) {
-                const uint32_t j = (uint32_t)(head + 4 * gi);
-                float4 s4, e4;
-                s4.x = piece_start(pc, j);     e4.x = f_add(s4.x, L.dt);
-                s4.y = piece_start(pc, j + 1); e4.y = f_add(s4.y, L.dt);
-                s4.z = piece_start(pc, j + 2); e4.z = f_add(s4.z, L.dt);
-                s4.w = piece_start(pc, j + 3); e4.w = f_add(s4.w, L.dt);
-                reinterpret_cast<float4*>(p.t_starts)[g0 + gi] = s4;
-                reinterpret_cast<float4*>(p.t_ends)[g0 + gi] = e4;
-                const longlong2 rr = make_longlong2(ray, ray);
-                reinterpret_cast<longlong2*>(p.ray_indices)[2 * (g0 + gi)] = rr;
-                reinterpret_cast<longlong2*>(p.ray_indices)[2 * (g0 + gi) + 1] = rr;
-            }
-            if (lane < tail) {
-                const Idx k = off + head + 4 * body_groups + lane;
-                const float ts = piece_start(pc, (uint32_t)(head + 4 * body_groups + lane));
-                p.ray_indices[k] = ray;
-                p.t_starts[k] = ts;
-                p.t_ends[k] = f_add(ts, L.dt);
-            }
-            off += c;
         }
     }
 }
@@ -1068,12 +1091,8 @@ struct PoolAppend {
         const cg::coalesced_group g = cg::coalesced_threads();
         uint32_t base = 0;
         if (g.thread_rank() == 0) base = atomicAdd(cursor, (uint32_t)g.size());
-        const uint32_t slot = g.shfl(base, 0) + (uint32_t)g.thread_rank();
-        if ((int64_t)slot < capacity) {
-            uint4* dst = reinterpret_cast<uint4*>(pool + slot);
-            dst[0] = make_uint4(ray, sample_off, n, __float_as_uint(t_first));
-            dst[1] = make_uint4(run_idx, tile, 0u, 0u);
-        }
+        store_run(pool, capacity, g.shfl(base, 0) + (uint32_t)g.thread_rank(), ray, tile, sample_off, n, t_first,
+                  run_idx);
     }
 };
 
@@ -1134,8 +1153,7 @@ __global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const Works
 {
     static_assert(kExpandLanes == 32, "one lane per sample of a piece");
     write_packed_info(ws, n_rays, packed_info);
-    int64_t n_runs = totals[1];
-    if (n_runs > ws.run_capacity) n_runs = ws.run_capacity;  // the host re-runs with a larger pool
+    const int64_t n_runs = pool_runs(ws, totals);
     const int lane = threadIdx.x & 31;
     const int64_t warp0 = ((int64_t)blockIdx.x * kExpandThreads + threadIdx.x) >> 5;
     const int64_t n_warps = ((int64_t)gridDim.x * kExpandThreads) >> 5;
@@ -1145,12 +1163,10 @@ __global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const Works
         float my_first = 0.f;
         int64_t my_k0 = 0;
         if (q < n_runs) {
-            const uint4 a = __ldg(reinterpret_cast<const uint4*>(ws.pool + q));
-            const uint32_t tile = __ldg(&ws.pool[q].tile);
+            const uint4 a = load_run(ws, q, my_k0);
             my_ray = a.x;
             my_n = a.z;
             my_first = __uint_as_float(a.w);
-            my_k0 = (int64_t)(ws.tile_base[tile] + ws.loc_samples[a.x]) + a.y;
         }
         for (int i = 0; i < 32; ++i) {
             const uint32_t n = __shfl_sync(0xffffffffu, my_n, i);
@@ -1270,6 +1286,35 @@ static void launch_march(const MarchParams& p, int tiles, int threads, cudaStrea
     march_kernel<kSingle, kSlots><<<tiles, threads, dyn, s>>>(p);
 }
 
+// The argument rules nfa_march and nfa_march_cone share.  True when there are rays to march; otherwise `status` is
+// what the call returns: an argument error or, with no rays, that of zeroing the totals (device and pinned mirror).
+static bool march_args_ok(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
+                          const float* far_planes, int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
+                          const uint64_t* words, const float* aabbs, bool have_sorted, float step_size,
+                          int64_t run_capacity, const void* workspace, int64_t* totals, int64_t* totals_host,
+                          cudaStream_t s, int32_t& status)
+{
+    if (n_rays < 0 || n_grids <= 0 || rx <= 0 || ry <= 0 || rz <= 0 || run_capacity < 0) status = NFA_ERR_ARG;
+    else if (run_capacity > (int64_t)UINT32_MAX || !(step_size > 0.0f)) status = NFA_ERR_UNSUPPORTED;
+    else if (!totals || (near_planes == nullptr) != (far_planes == nullptr)) status = NFA_ERR_ARG;
+    else if (n_rays == 0) {
+        if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
+        status = (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
+    } else if (!rays_o || !rays_d || !words || !aabbs || !workspace || (!have_sorted && n_grids != 1))
+        status = NFA_ERR_ARG;  // (nested levels need the sorted crossings)
+    else
+        return true;
+    return false;
+}
+
+// Expand grid for `threads` threads: at least one CTA, at most the 8 CTAs of kExpandThreads resident per SM.
+static inline int expand_grid(int64_t threads)
+{
+    const int64_t ctas = (threads + kExpandThreads - 1) / kExpandThreads;
+    const int64_t cap = kNumSMs * 8;
+    return (int)(ctas < 1 ? 1 : (ctas < cap ? ctas : cap));
+}
+
 extern "C" {
 
 // measurement aid, not part of the product path: per-warp time stamps of the next nfa_march launches go to
@@ -1354,20 +1399,12 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
                   int64_t run_capacity, void* workspace, int64_t* totals, int64_t* totals_host,
                   float* terminate_planes, nfa_stream_t stream)
 {
-    if (n_rays < 0 || n_grids <= 0 || rx <= 0 || ry <= 0 || rz <= 0 || run_capacity < 0) return NFA_ERR_ARG;
-    if (run_capacity > (int64_t)UINT32_MAX) return NFA_ERR_UNSUPPORTED;
-    if (!(step_size > 0.0f)) return NFA_ERR_UNSUPPORTED;
-    if (!totals) return NFA_ERR_ARG;
     cudaStream_t s = (cudaStream_t)stream;
-    if ((near_planes == nullptr) != (far_planes == nullptr)) return NFA_ERR_ARG;
-    if (n_rays == 0) {
-        if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
-        return (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
-    }
-    if (!rays_o || !rays_d || !words || !aabbs || !workspace)
-        return NFA_ERR_ARG;
     const bool have_sorted = t_sorted && t_indices && hits;
-    if (!have_sorted && n_grids != 1) return NFA_ERR_ARG;
+    int32_t status;
+    if (!march_args_ok(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, aabbs, have_sorted,
+                       step_size, run_capacity, workspace, totals, totals_host, s, status))
+        return status;
     MarchParams p;
     p.n_rays = n_rays;
     p.rays_o = rays_o;
@@ -1416,13 +1453,6 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
     return launch_status();
 }
 
-static inline int expand_grid(int64_t run_capacity)
-{
-    const int64_t ctas = (run_capacity * 32 + kExpandThreads - 1) / kExpandThreads;
-    const int64_t cap = kNumSMs * 8;  // 8 resident CTAs of 256 threads per SM
-    return (int)(ctas < 1 ? 1 : (ctas < cap ? ctas : cap));
-}
-
 int32_t nfa_expand_samples(int32_t n_rays, int64_t run_capacity, const void* workspace, const int64_t* totals,
                            float step_size, int64_t capacity, int64_t* packed_info, int64_t* ray_indices,
                            float* t_starts, float* t_ends, nfa_stream_t stream)
@@ -1432,28 +1462,13 @@ int32_t nfa_expand_samples(int32_t n_rays, int64_t run_capacity, const void* wor
     if (!workspace || !packed_info || !totals) return NFA_ERR_ARG;
     if (capacity > 0 && (!ray_indices || !t_starts || !t_ends)) return NFA_ERR_ARG;
     if ((((uintptr_t)packed_info) & 15u) != 0) return NFA_ERR_ARG;
-    const Workspace ws = ws_view(const_cast<void*>(workspace), n_rays, run_capacity);
-    cudaStream_t s = (cudaStream_t)stream;
-    const uintptr_t al = (uintptr_t)ray_indices | (uintptr_t)t_starts | (uintptr_t)t_ends;
-    const bool expand = capacity > 0 && run_capacity > 0;
-    // the vectorised kernel writes packed_info itself (from what the march left in the workspace); the offsets pass
-    // only runs in front of the scalar fallback (unaligned outputs) or when there is nothing to expand
-    if (!expand || (al & 15u) != 0) offsets_kernel<false><<<ws.n_tiles, ws.tile_rays, 0, s>>>(n_rays, ws, packed_info, nullptr);
-    if (expand) {
-        ExpandParams p = {};
-        p.ws = ws;
-        p.n_rays = n_rays;
-        p.totals = totals;
-        p.step_size = step_size;
-        p.sample_capacity = capacity;
-        p.sm_packed_info = packed_info;
-        p.packed_out = packed_info;
-        p.ray_indices = ray_indices;
-        p.t_starts = t_starts;
-        p.t_ends = t_ends;
-        if ((al & 15u) != 0) expand_runs_kernel<false><<<expand_grid(run_capacity), kExpandThreads, 0, s>>>(p);
-        else expand_runs_vec_kernel<<<expand_grid(run_capacity), kExpandThreads, 0, s>>>(p);
-    }
+    const SamplesParams p = {ws_view(const_cast<void*>(workspace), n_rays, run_capacity), n_rays, totals, step_size,
+                             capacity, packed_info, ray_indices, t_starts, t_ends};
+    // a warp per run, and a thread per ray for packed_info (written even when nothing is expanded)
+    const int grid = expand_grid(32 * run_capacity > n_rays ? 32 * run_capacity : n_rays);
+    const bool vec = (((uintptr_t)ray_indices | (uintptr_t)t_starts | (uintptr_t)t_ends) & 15u) == 0;
+    const cudaStream_t s = (cudaStream_t)stream;
+    (vec ? expand_samples_kernel<true> : expand_samples_kernel<false>)<<<grid, kExpandThreads, 0, s>>>(p);
     return launch_status();
 }
 
@@ -1471,24 +1486,12 @@ int32_t nfa_expand_intervals(int32_t n_rays, int64_t run_capacity, const void* w
     if (((((uintptr_t)iv_packed_info) | ((uintptr_t)sm_packed_info)) & 15u) != 0) return NFA_ERR_ARG;
     const Workspace ws = ws_view(const_cast<void*>(workspace), n_rays, run_capacity);
     cudaStream_t s = (cudaStream_t)stream;
-    offsets_kernel<true><<<ws.n_tiles, ws.tile_rays, 0, s>>>(n_rays, ws, sm_packed_info, iv_packed_info);
+    offsets_kernel<<<ws.n_tiles, ws.tile_rays, 0, s>>>(n_rays, ws, sm_packed_info, iv_packed_info);
     if (edge_capacity > 0 && run_capacity > 0) {
-        ExpandParams p = {};
-        p.ws = ws;
-        p.totals = totals;
-        p.step_size = step_size;
-        p.sample_capacity = sample_capacity;
-        p.sm_packed_info = sm_packed_info;
-        p.ray_indices = sm_ray_indices;
-        p.edge_capacity = edge_capacity;
-        p.iv_packed_info = iv_packed_info;
-        p.iv_vals = iv_vals;
-        p.iv_ray_indices = iv_ray_indices;
-        p.iv_is_left = iv_is_left;
-        p.iv_is_right = iv_is_right;
-        p.sm_vals = sm_vals;
-        p.sm_is_valid = sm_is_valid;
-        expand_runs_kernel<true><<<expand_grid(run_capacity), kExpandThreads, 0, s>>>(p);
+        const IntervalsParams p = {ws, totals, step_size,
+                                   sm_packed_info, sm_ray_indices, sm_vals, sm_is_valid, sample_capacity,
+                                   iv_packed_info, iv_ray_indices, iv_vals, iv_is_left, iv_is_right, edge_capacity};
+        expand_intervals_kernel<<<expand_grid(32 * run_capacity), kExpandThreads, 0, s>>>(p);
     }
     return launch_status();
 }
@@ -1500,19 +1503,13 @@ int32_t nfa_march_cone(int32_t n_rays, const float* rays_o, const float* rays_d,
                        float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
                        int64_t* totals_host, nfa_stream_t stream)
 {
-    if (n_rays < 0 || n_grids <= 0 || rx <= 0 || ry <= 0 || rz <= 0 || run_capacity < 0) return NFA_ERR_ARG;
-    if (run_capacity > (int64_t)UINT32_MAX) return NFA_ERR_UNSUPPORTED;
-    if (!(step_size > 0.0f)) return NFA_ERR_UNSUPPORTED;
-    if (!totals) return NFA_ERR_ARG;
-    if ((near_planes == nullptr) != (far_planes == nullptr)) return NFA_ERR_ARG;
     cudaStream_t s = (cudaStream_t)stream;
-    if (n_rays == 0) {
-        if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
-        return (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
-    }
-    if (!rays_o || !rays_d || !words || !coarse || !aabbs || !workspace) return NFA_ERR_ARG;
     const bool have_sorted = t_sorted && t_indices && hits;
-    if (!have_sorted && n_grids != 1) return NFA_ERR_ARG;
+    int32_t status;
+    if (!march_args_ok(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, aabbs, have_sorted,
+                       step_size, run_capacity, workspace, totals, totals_host, s, status))
+        return status;
+    if (!coarse) return NFA_ERR_ARG;
     ConeParams p;
     p.n_rays = n_rays;
     p.rays_o = rays_o;
@@ -1548,11 +1545,8 @@ int32_t nfa_expand_cone_samples(int32_t n_rays, int64_t run_capacity, const void
     if (capacity > 0 && (!ray_indices || !t_starts || !t_ends)) return NFA_ERR_ARG;
     if ((((uintptr_t)packed_info) & 15u) != 0) return NFA_ERR_ARG;
     const Workspace ws = ws_view(const_cast<void*>(workspace), n_rays, run_capacity);
-    // enough threads for the packed_info prologue and for every run of the pool
-    const int64_t work = run_capacity > n_rays ? run_capacity : n_rays;
-    const int64_t ctas = (work + kExpandThreads - 1) / kExpandThreads;
-    const int64_t cap = kNumSMs * 8;
-    const int grid = (int)(ctas < 1 ? 1 : (ctas < cap ? ctas : cap));
+    // a lane per run, and a thread per ray for packed_info
+    const int grid = expand_grid(run_capacity > n_rays ? run_capacity : n_rays);
     expand_cone_kernel<<<grid, kExpandThreads, 0, (cudaStream_t)stream>>>(ws, n_rays, totals, step_size, cone_angle,
                                                                           capacity, packed_info, ray_indices, t_starts,
                                                                           t_ends);

@@ -26,8 +26,8 @@ def demangle(n):
 print("# SASS of", so, "(cuobjdump -sass, sm_90a)\n")
 for name, ins in funcs.items():
     d = demangle(name)
-    if not any(k in d for k in ("march_kernel<true, false, 16>", "march_kernel<(bool)1, (bool)0, (int)16>", "Cfg<false, true, true>", "expand_runs_vec",
-                                "occ_threshold_pack", "vis_mask_kernel<(bool)0>")):
+    if not any(k in d for k in ("march_kernel<true, 16>", "march_kernel<(bool)1, (int)16>", "Cfg<false, true, true>",
+                                "expand_samples_kernel", "occ_threshold_pack", "vis_mask_kernel<(bool)0>")):
         continue
     hist = collections.Counter(re.sub(r"^@!?U?P\d+\s+", "", t).split()[0].split(".")[0] for _, t in ins)
     print(f"## {d}\n{len(ins)} instructions; top mnemonics: " + ", ".join(f"{k} {v}" for k, v in hist.most_common(14)))

@@ -438,9 +438,10 @@ def _march_abi(name):
     return dict(R=R, cap=cap, ws=ws, tot=tot, step=step, n=n, runs=runs, keep=(occ, o, d, a, tsrt, tidx, hits))
 
 
-def _expand_samples(m, capacity, offsets=(0, 0)):
+def _expand_samples(m, capacity, offsets=(0, 0), run_capacity=None):
     """nfa_expand_samples into sentinel-filled allocations of n + GUARD (+ offset) elements; the views start
-    `offsets` = (float elements, int64 elements) into them.  Returns (packed_info, the three allocations, views)."""
+    `offsets` = (float elements, int64 elements) into them.  `run_capacity` defaults to the march's pool size.
+    Returns (packed_info, the three allocations, views)."""
     from nerfacc_b200 import _lib
     n, fo, io = m["n"], offsets[0], offsets[1]
     ts_buf = torch.full((n + GUARD + fo,), F_SENT, device=dev)
@@ -448,7 +449,8 @@ def _expand_samples(m, capacity, offsets=(0, 0)):
     ri_buf = torch.full((n + GUARD + io,), I_SENT, dtype=torch.int64, device=dev)
     pi = torch.full((m["R"], 2), I_SENT, dtype=torch.int64, device=dev)
     ts, te, ri = ts_buf[fo:], te_buf[fo:], ri_buf[io:]
-    _lib.call("nfa_expand_samples", torch.device(dev), m["R"], m["cap"], m["ws"].data_ptr(), m["tot"].data_ptr(),
+    run_capacity = m["cap"] if run_capacity is None else run_capacity
+    _lib.call("nfa_expand_samples", torch.device(dev), m["R"], run_capacity, m["ws"].data_ptr(), m["tot"].data_ptr(),
               m["step"], capacity, pi.data_ptr(), ri.data_ptr(), ts.data_ptr(), te.data_ptr())
     torch.cuda.synchronize()
     return N(pi), (N(ri_buf), N(ts_buf), N(te_buf)), (N(ri), N(ts), N(te))
@@ -459,7 +461,8 @@ def _expand_samples(m, capacity, offsets=(0, 0)):
 def test_expand_samples_clipped_and_unaligned(orc, name):
     """nfa_expand_samples with capacity n - k (the speculative call whose batch outgrew the hint): the first
     `capacity` elements are the full result, nothing at or past `capacity` is written, packed_info is complete.
-    With outputs 4 / 8 bytes off 16-byte alignment (scalar kernel + offsets pass) the result is byte-identical."""
+    Capacity 0 (k = n) and an empty run pool (run_capacity 0) write packed_info and nothing else.  With outputs
+    4 / 8 bytes off 16-byte alignment (element-wise stores) the result is byte-identical."""
     bins, aabbs, ro, rd, step, far = scene(name)
     m = _march_abi(name)
     n = m["n"]
@@ -471,16 +474,17 @@ def test_expand_samples_clipped_and_unaligned(orc, name):
     np.testing.assert_array_equal(ts, o_ts)
     np.testing.assert_array_equal(te, o_te)
     full = (ri, ts, te)
-    for offsets in ((0, 0), (1, 1), (2, 1), (1, 0)):        # 4- / 8-byte offsets: the scalar kernel
-        for k in (0, 1, 3, 4, 5, n // 2):
-            cap = n - k
-            pk, bufs, views = _expand_samples(m, cap, offsets)
-            msg = f"offsets={offsets} capacity=n-{k}"
+    for offsets in ((0, 0), (1, 1), (2, 1), (1, 0)):        # 4- / 8-byte offsets: the element-wise stores
+        # (capacity, run_capacity, elements written)
+        cases = [(n - k, m["cap"], n - k) for k in (0, 1, 3, 4, 5, n // 2, n)] + [(n, 0, 0)]
+        for cap, run_cap, kept in cases:
+            pk, bufs, views = _expand_samples(m, cap, offsets, run_cap)
+            msg = f"offsets={offsets} capacity={cap} (n={n}) run_capacity={run_cap}"
             np.testing.assert_array_equal(pk, pi, err_msg=msg)
             for got, want, buf, off, sent in zip(views, full, bufs, (offsets[1], offsets[0], offsets[0]),
                                                  (I_SENT, F_SENT, F_SENT)):
-                assert got[:cap].tobytes() == want[:cap].tobytes(), msg
-                assert (got[cap:] == sent).all(), f"{msg}: written at or past the capacity"
+                assert got[:kept].tobytes() == want[:kept].tobytes(), msg
+                assert (got[kept:] == sent).all(), f"{msg}: written at or past index {kept}"
                 assert (buf[:off] == sent).all(), f"{msg}: written before the output"
 
 

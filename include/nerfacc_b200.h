@@ -28,7 +28,7 @@ extern "C" {
 #define NFA_ERR_ARG (-1)         /* null pointer / negative size / inconsistent sizes */
 #define NFA_ERR_UNSUPPORTED (-2) /* valid request outside what this build implements */
 
-#define NFA_ABI_VERSION 12
+#define NFA_ABI_VERSION 13
 
 typedef void* nfa_stream_t; /* cudaStream_t */
 
@@ -283,6 +283,53 @@ int32_t nfa_scan_by_key(int64_t n, const int64_t* keys, const float* in, float* 
 int64_t nfa_pack_info_workspace_bytes(int32_t n_rays);
 int32_t nfa_pack_info(int64_t n, const int64_t* ray_indices, int32_t n_rays, int64_t* packed_info,
                       void* workspace, nfa_stream_t stream);
+
+/* ----------------------------------------------------------------------- */
+/* Packed <-> padded per-ray layout (nerfacc 0.3's unpack_info / unpack_data / pack_data, removed in 0.5.0,     */
+/* CHANGELOG.md:38; in 0.5 code the `data[mask]` / index-arithmetic ATen compositions written in their place)   */
+/* ----------------------------------------------------------------------- */
+
+/* Byte movers: a row is `row_bytes` bytes (element size x elements per sample), copied in the largest of
+ * 16 / 8 / 4 / 2 / 1-byte units that divides row_bytes and every data pointer, so any dtype is bit-exact.
+ * packed rows [n_packed]; padded rows [n_rays, n_per_ray]; packed_info [n_rays, 2] = (start, count), counts < 0
+ * read as 0.  Packed positions outside [0, n_packed) are neither read nor written.
+ * "In order" below means start_r >= start_{r-1} + count_{r-1} for every r (every packed_info this library returns);
+ * the library checks it on the device.  workspace: nfa_chunk_order_workspace_bytes() bytes, no initial value. */
+int64_t nfa_chunk_order_workspace_bytes(void);
+
+/* replaces: unpack_info(packed_info, n_samples) (0.3) / torch.repeat_interleave(arange(n_rays), counts).
+ *   ray_indices [n_samples] int64: r on chunk r, -1 where no chunk lands.  Chunks in order: one store pass
+ *   (each ray also writes the gap behind its chunk); otherwise a -1 fill pass first.  Chunks must not overlap. */
+int32_t nfa_unpack_info(int32_t n_rays, const int64_t* packed_info, int64_t n_samples, int64_t* ray_indices,
+                        void* workspace, nfa_stream_t stream);
+
+/* replaces: unpack_data(packed_info, data, n_samples, pad_value) (0.3) / torch.full + masked index assignment.
+ *   padded[r, j] = packed[start_r + j] for j < min(count_r, n_per_ray) (and inside [0, n_packed)), else the
+ *   row at `pad_row` (device memory, row_bytes bytes).  Every padded row is written by the one kernel.
+ *   packed may be NULL when n_packed == 0. */
+int32_t nfa_unpack_rows(int32_t n_rays, const int64_t* packed_info, int64_t n_packed, int64_t n_per_ray,
+                        int64_t row_bytes, const void* packed, const void* pad_row, void* padded, nfa_stream_t stream);
+
+/* replaces: the backward of the above (a scatter of the padded gradient into zeros).
+ *   packed[start_r + j] = padded[r, j] for j < min(count_r, n_per_ray); every other packed row (truncated, or in
+ *   no chunk) is zero.  Chunks in order: one pass; otherwise a zero fill pass first. */
+int32_t nfa_pack_rows(int32_t n_rays, const int64_t* packed_info, int64_t n_packed, int64_t n_per_ray,
+                      int64_t row_bytes, const void* padded, void* packed, void* workspace, nfa_stream_t stream);
+
+/* replaces: mask.sum(-1) of pack_data (0.3).  counts [n_rays] int64 = number of nonzero bytes in each row of
+ *   mask [n_rays, n_per_ray] (bool bytes); nfa_counts_to_packed_info turns them into packed_info. */
+int32_t nfa_mask_counts(int32_t n_rays, int64_t n_per_ray, const uint8_t* mask, int64_t* counts, nfa_stream_t stream);
+
+/* replaces: data[mask] of pack_data (0.3) and its backward (a masked scatter into zeros).
+ *   Row j of ray r is kept iff mask[r, j]; the kept rows of ray r are packed rows start_r, start_r + 1, ... in j
+ *   order (packed_info from nfa_counts_to_packed_info of nfa_mask_counts).
+ *   nfa_pack_masked:   padded -> packed (only kept rows written).
+ *   nfa_unpack_masked: packed -> padded, every padded row written (zero where the mask is false); packed may be
+ *                      NULL when no mask byte is set. */
+int32_t nfa_pack_masked(int32_t n_rays, int64_t n_per_ray, int64_t row_bytes, const uint8_t* mask,
+                        const int64_t* packed_info, const void* padded, void* packed, nfa_stream_t stream);
+int32_t nfa_unpack_masked(int32_t n_rays, int64_t n_per_ray, int64_t row_bytes, const uint8_t* mask,
+                          const int64_t* packed_info, const void* packed, void* padded, nfa_stream_t stream);
 
 /* replaces: the visibility branch of OccGridEstimator.sampling (nerfacc/estimators/occ_grid.py:180-220):
  *   render_visibility_from_density / _from_alpha (volrend.py:379-494; native exclusive_sum / exclusive_prod on

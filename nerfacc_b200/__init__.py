@@ -12,7 +12,7 @@ from .version import __version__
 
 _EXPORTS = {
     scan: ("inclusive_prod", "exclusive_prod", "inclusive_sum", "exclusive_sum"),
-    pack: ("pack_info",),
+    pack: ("pack_info", "unpack_info", "pack_data", "unpack_data"),
     volrend: ("render_visibility_from_alpha", "render_visibility_from_density", "render_weight_from_alpha",
               "render_weight_from_density", "render_transmittance_from_alpha", "render_transmittance_from_density",
               "accumulate_along_rays", "accumulate_along_rays_", "rendering"),

@@ -75,9 +75,16 @@ SIGNATURES = {
     "nfa_mailbox_sum": (_c_i32, [_c_ptr, _c_i32, _c_i32, C.c_uint32, _c_f32, _c_ptr, _c_ptr, _c_ptr]),
     "nfa_pack_info_workspace_bytes": (_c_i64, [_c_i32]),
     "nfa_pack_info": (_c_i32, [_c_i64, _c_ptr, _c_i32, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_chunk_order_workspace_bytes": (_c_i64, []),
+    "nfa_unpack_info": (_c_i32, [_c_i32, _c_ptr, _c_i64, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_unpack_rows": (_c_i32, [_c_i32, _c_ptr, _c_i64, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_pack_rows": (_c_i32, [_c_i32, _c_ptr, _c_i64, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_mask_counts": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_pack_masked": (_c_i32, [_c_i32, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_unpack_masked": (_c_i32, [_c_i32, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
 }
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 _lib = None
 launches = 0  # number of native kernel-launching calls made through this module (bench.py reports it)

@@ -28,7 +28,7 @@ extern "C" {
 #define NFA_ERR_ARG (-1)         /* null pointer / negative size / inconsistent sizes */
 #define NFA_ERR_UNSUPPORTED (-2) /* valid request outside what this build implements */
 
-#define NFA_ABI_VERSION 13
+#define NFA_ABI_VERSION 14
 
 typedef void* nfa_stream_t; /* cudaStream_t */
 
@@ -63,7 +63,7 @@ int32_t nfa_intersect_sorted(int32_t n_rays, const float* rays_o, const float* r
  * words  [nfa_occ_words()]        uint64, one per 4x4x4-cell brick,
  * coarse [nfa_occ_coarse_words()] uint32, two bits per brick, 16 bricks per word: bit 0 "some cell set",
  *                                 bit 1 "all 64 cells set" (0 empty, 1 mixed, 3 full); read by
- *                                 nfa_traverse_generic only,
+ *                                 nfa_traverse_generic and the growing-step nfa_march,
  * bounds [n_grids * 6]            int32, per level min xyz / max xyz (inclusive, brick units) of the
  *                                 non-empty bricks; min > max when the level is empty. */
 int64_t nfa_occ_words(int32_t n_grids, int32_t rx, int32_t ry, int32_t rz);
@@ -91,17 +91,19 @@ int32_t nfa_counts_to_packed_info(int32_t n_rays, const int64_t* counts, int64_t
                                   nfa_stream_t stream);
 
 /* Measurement aid (scripts/march_trace.py), not used by the product path: per-warp time stamps of the following
- * nfa_march launches are written to `buffer` (8 x uint64 per warp, n_tiles x 16 warps); null switches it off. */
+ * constant-step (cone_angle == 0) nfa_march launches are written to `buffer` (8 x uint64 per warp, n_tiles x 16
+ * warps); null switches it off.  Growing-step launches write none. */
 void nfa_debug_set_march_trace(void* buffer);
 
 /* ----------------------------------------------------------------------- */
-/* Grid traversal, constant step (cone_angle == 0, step_size > 0)           */
+/* Grid traversal by runs (step_size > 0)                                   */
 /* ----------------------------------------------------------------------- */
 
 /* replaces: traverse_grids(...) nerfacc/cuda/csrc/nerfacc.cpp:75-96, grid.cu:320-474
- *   (kernel :68-282) for the two-pass (exact allocation) mode.
+ *   (kernel :68-282) for the two-pass (exact allocation) mode; with the expand calls below, also the
+ *   `vals[is_left]`, `vals[is_right]` of nerfacc/estimators/occ_grid.py:174-177.
  *
- * nfa_march: one DDA pass per ray.  Appends every run (t_first, n) of consecutive
+ * nfa_march: one pass per ray.  Appends every run (t_first, n) of consecutive
  *   samples to a pool inside `workspace` (capacity `run_capacity` runs) and writes per-ray
  *   sample / run counts there; the totals
  *     totals[0] = n_samples, [1] = n_runs, [2] = run_capacity used, [3] = rays whose
@@ -112,32 +114,39 @@ void nfa_debug_set_march_trace(void* buffer);
  *   far_plane for every ray (reference occ_grid.py:154-155 builds those tensors with full_like).  If totals[1] > run_capacity the pool
  *   overflowed: call again with a larger pool (counts and totals are still exact).
  *   t_sorted / t_indices / hits may be NULL when n_grids == 1 (crossings are then
- *   computed in the kernel).  terminate_planes [n_rays] may be NULL.  `words` and `bounds` come from
- *   nfa_occ_pack; `bounds` (nullable) lets single-level calls without terminate planes jump over /
- *   stop after empty space.
+ *   computed in the kernel).  `words`, `coarse` and `bounds` come from nfa_occ_pack.
  *   workspace: nfa_march_workspace_bytes(n_rays, run_capacity) bytes whose first 64
- *   bytes are zero on first use (the kernels leave it reusable). */
+ *   bytes are zero on first use (the kernels leave it reusable).
+ *   cone_angle (>= 0) selects the walk:
+ *   == 0  constant step, one DDA pass.  `coarse` is not read; `bounds` (nullable) lets single-level calls
+ *         without terminate planes jump over / stop after empty space; terminate_planes [n_rays] may be NULL.
+ *   >  0  growing step (unbounded scenes), dt = clamp(t * cone_angle, step_size, 1e10), sample by sample in the
+ *         reference's order of operations.  `coarse` is required, `bounds` is not read, terminate_planes must be
+ *         NULL.  A ray whose marching variable stops advancing (t + dt == t) ends there without an error, as in
+ *         nfa_traverse_generic: totals[3] is always 0. */
 int64_t nfa_march_workspace_bytes(int32_t n_rays, int64_t run_capacity);
 int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d,
                   const float* near_planes, const float* far_planes, float near_plane, float far_plane,
                   int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
-                  const uint64_t* words, const int32_t* bounds, const float* aabbs,
+                  const uint64_t* words, const uint32_t* coarse, const int32_t* bounds, const float* aabbs,
                   const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,
-                  float step_size, int64_t run_capacity, void* workspace, int64_t* totals,
+                  float step_size, float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
                   int64_t* totals_host, float* terminate_planes, nfa_stream_t stream);
 
 /* nfa_expand_samples: runs -> packed (ray_indices, t_starts, t_ends) + packed_info.
  *   replaces the fill pass plus `vals[is_left]`, `vals[is_right]` of
  *   nerfacc/estimators/occ_grid.py:174-177.  `totals` is the device array nfa_march
- *   filled.  Elements at index >= capacity are not written (the caller re-runs with a
- *   larger buffer).  packed_info: [n_rays, 2] = (chunk_start, chunk_cnt), always written by this call
- *   (in the one kernel it launches, also when capacity or run_capacity is 0). */
+ *   filled; step_size and cone_angle must be the march's.  Elements at index >= capacity are not written (the
+ *   caller re-runs with a larger buffer).  packed_info: [n_rays, 2] = (chunk_start, chunk_cnt), 16-byte aligned,
+ *   always written by this call (in the one kernel it launches, also when capacity or run_capacity is 0).
+ *   cone_angle == 0: every run computed from the lattice closed form.  cone_angle > 0: every run replayed as
+ *   t_{j+1} = t_j + dt(t_j) from its t_first (the same float operations as the march, so the same bits). */
 int32_t nfa_expand_samples(int32_t n_rays, int64_t run_capacity, const void* workspace,
-                           const int64_t* totals, float step_size, int64_t capacity,
+                           const int64_t* totals, float step_size, float cone_angle, int64_t capacity,
                            int64_t* packed_info, int64_t* ray_indices, float* t_starts, float* t_ends,
                            nfa_stream_t stream);
 
-/* nfa_expand_intervals: runs -> the RaySegmentsSpec pair traverse_grids returns
+/* nfa_expand_intervals: runs of a constant-step nfa_march -> the RaySegmentsSpec pair traverse_grids returns
  *   (nerfacc/cuda/csrc/include/data_spec.hpp:6-16, nerfacc/data_specs.py:12-180):
  *   intervals {vals, ray_indices, is_left, is_right, packed_info} with n_samples + n_runs
  *   edges, samples {vals = midpoints, ray_indices, is_valid, packed_info}. */
@@ -148,35 +157,6 @@ int32_t nfa_expand_intervals(int32_t n_rays, int64_t run_capacity, const void* w
                              uint8_t* iv_is_left, uint8_t* iv_is_right,
                              int64_t* sm_packed_info, float* sm_vals, int64_t* sm_ray_indices,
                              uint8_t* sm_is_valid, nfa_stream_t stream);
-
-/* ----------------------------------------------------------------------- */
-/* Grid traversal, growing step (cone_angle > 0, step_size > 0)             */
-/* ----------------------------------------------------------------------- */
-
-/* replaces: traverse_grids(..., cone_angle > 0) nerfacc/cuda/csrc/grid.cu:68-282 (launches :320-474) followed by
- *   `vals[is_left]`, `vals[is_right]` of nerfacc/estimators/occ_grid.py:174-177 -- OccGridEstimator.sampling for
- *   unbounded scenes, where the step grows with the distance: dt = clamp(t * cone_angle, step_size, 1e10).
- *
- * nfa_march_cone: one thread per ray marches sample by sample in the reference's order of operations and appends
- *   every run (t_first, n) of consecutive samples to the run pool of `workspace`, in nfa_march's record format, with
- *   nfa_march's per-ray counts, tile sums and totals (so nfa_march_workspace_bytes sizes the workspace and the
- *   run-pool overflow rule is the same).  Arguments as nfa_march, plus `coarse` (nfa_occ_pack) and cone_angle; no
- *   terminate planes.  A ray whose marching variable stops advancing (t + dt == t) ends there without an error, as in
- *   nfa_traverse_generic: totals[3] is always 0.
- * nfa_expand_cone_samples: runs -> packed (ray_indices, t_starts, t_ends) + packed_info, each run replayed as
- *   t_{j+1} = t_j + dt(t_j) from its t_first (the same float operations as the march, so the same bits).  Same
- *   arguments and capacity rule as nfa_expand_samples, plus cone_angle; packed_info is always written. */
-int32_t nfa_march_cone(int32_t n_rays, const float* rays_o, const float* rays_d,
-                       const float* near_planes, const float* far_planes, float near_plane, float far_plane,
-                       int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
-                       const uint64_t* words, const uint32_t* coarse, const float* aabbs,
-                       const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,
-                       float step_size, float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
-                       int64_t* totals_host, nfa_stream_t stream);
-int32_t nfa_expand_cone_samples(int32_t n_rays, int64_t run_capacity, const void* workspace,
-                                const int64_t* totals, float step_size, float cone_angle, int64_t capacity,
-                                int64_t* packed_info, int64_t* ray_indices, float* t_starts, float* t_ends,
-                                nfa_stream_t stream);
 
 /* nfa_traverse_generic: the remaining modes of traverse_grids (nerfacc.cpp:75-96, grid.cu:320-474) --
  *   cone_angle > 0, step_size <= 0 (one sample per occupied cell), traverse_steps_limit, over_allocate

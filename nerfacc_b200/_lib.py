@@ -35,16 +35,11 @@ SIGNATURES = {
     "nfa_debug_set_march_trace": (None, [_c_ptr]),
     "nfa_march_workspace_bytes": (_c_i64, [_c_i32, _c_i64]),
     "nfa_march": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i32, _c_i32, _c_i32, _c_i32,
-                           _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_ptr, _c_ptr,
-                           _c_ptr, _c_ptr, _c_ptr]),
-    "nfa_expand_samples": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr,
-                                    _c_ptr]),
+                           _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i64, _c_ptr,
+                           _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_expand_samples": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i64, _c_ptr, _c_ptr, _c_ptr,
+                                    _c_ptr, _c_ptr]),
     "nfa_expand_intervals": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_i64, _c_i64] + [_c_ptr] * 10),
-    "nfa_march_cone": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i32, _c_i32, _c_i32, _c_i32,
-                                _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i64, _c_ptr, _c_ptr,
-                                _c_ptr, _c_ptr]),
-    "nfa_expand_cone_samples": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i64, _c_ptr, _c_ptr, _c_ptr,
-                                         _c_ptr, _c_ptr]),
     "nfa_traverse_generic": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_i32, _c_i32, _c_i32, _c_i32,
                                       _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_f32, _c_f32, _c_i32, _c_i32]
                              + [_c_ptr] * 14),
@@ -84,7 +79,7 @@ SIGNATURES = {
     "nfa_unpack_masked": (_c_i32, [_c_i32, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
 }
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 _lib = None
 launches = 0  # number of native kernel-launching calls made through this module (bench.py reports it)

@@ -5,8 +5,8 @@
 // (/root/reference/nerfacc/cuda/csrc/grid.cu:68-282, launches :364-470).  One thread marches one
 // ray sample by sample, in the reference's order of operations; a first pass counts, a second
 // fills at the scanned offsets (or one pass into fixed-stride slots when over-allocating).
-// The same walk with a run sink (RunSink) feeds nfa_march_cone / nfa_expand_cone_samples, the growing-step
-// sampling path: runs instead of samples, one pass, replayed by the expand kernel.
+// The same walk with a run sink (RunSink) feeds nfa_march / nfa_expand_samples with cone_angle > 0, the
+// growing-step sampling path: runs instead of samples, one pass, replayed by the expand kernel.
 // Reuses the DDA set-up, slab test, occupancy words and crossing iterators of march.cuh.
 // Host+device so that tests/host_sim can check it against the oracle on the CPU.
 #pragma once
@@ -89,7 +89,7 @@ NFA_HD void generic_emit(GenericOut& o, float t_last, float t_next, bool continu
     o.n_samples += 1;
 }
 
-// Run sink (nfa_march_cone): the samples of a ray as runs -- maximal chains of samples emitted with `continuous`
+// Run sink (march_cone_kernel): the samples of a ray as runs -- maximal chains of samples emitted with `continuous`
 // set, each sample starting where the previous one ended.  An emission with `continuous == false` opens a run and
 // the continuous ones that follow extend it; `continuous` is not reset between grid levels, so a run can span
 // levels.  Inside a run every sample is [t, cone_next(t)] of the previous sample's end (the emission loop below

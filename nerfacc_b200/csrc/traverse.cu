@@ -22,7 +22,8 @@
 //                     per-ray sample and run counts into both packed_infos (ray-ordered offsets, so ray_indices
 //                     stay sorted), then one warp per run writes the edges and the samples.
 //   march_cone_kernel / expand_cone_kernel
-//                     sampling() with growing steps (cone_angle > 0): 1 thread / ray walks sample by sample
+//                     what nfa_march / nfa_expand_samples launch in place of the two above for growing steps
+//                     (cone_angle > 0): 1 thread / ray walks sample by sample
 //                     (march_generic.cuh) into the same run pool, counts and tile sums as march_kernel;
 //                     a warp replays 32 runs one after the other, one lane per sample of a 32-sample piece.
 //   generic_traverse_kernel  every other traverse_grids mode (march_generic.cuh).
@@ -232,6 +233,8 @@ __global__ void occ_bounds_init_kernel(int32_t* bounds, int n_grids)
 // ---------------------------------------------------------------------------
 // march
 // ---------------------------------------------------------------------------
+// Arguments of both march kernels: march_kernel (constant step) reads bounds, lat_table, trace and terminate,
+// march_cone_kernel (growing step) reads coarse and cone_angle.
 struct MarchParams {
     int32_t n_rays;
     const float* rays_o;
@@ -241,12 +244,13 @@ struct MarchParams {
     float near_plane, far_plane;
     OccGeom g;
     const uint64_t* words;
-    const int32_t* bounds;  // occupied-brick bounding boxes (nullable)
+    const uint32_t* coarse;  // brick class mip
+    const int32_t* bounds;   // occupied-brick bounding boxes (nullable)
     const float* aabbs;
-    const float* t_sorted;
+    const float* t_sorted;  // null: one level, crossings computed in the kernel
     const int64_t* t_indices;
     const uint8_t* hits;
-    float step_size;
+    float step_size, cone_angle;
     LatTable lat_table;   // lattice points at the binade starts, from the uniform near plane (n = 0: none)
     unsigned long long* trace;  // measurement aid (nfa_debug_set_march_trace): 8 x u64 per warp, or null
     Workspace ws;
@@ -837,6 +841,7 @@ struct SamplesParams {
     int32_t n_rays;
     const int64_t* totals;  // device copy of the march totals ([1] = number of runs)
     float step_size;
+    float cone_angle;  // expand_cone_kernel only
     int64_t capacity;
     int64_t* packed_info;
     int64_t* ray_indices;
@@ -1060,26 +1065,6 @@ __global__ void __launch_bounds__(128) generic_traverse_kernel(const GenericPara
 // ---------------------------------------------------------------------------
 // growing steps (cone_angle > 0): walk -> runs -> expand, the layout of the constant-step path
 // ---------------------------------------------------------------------------
-struct ConeParams {
-    int32_t n_rays;
-    const float* rays_o;
-    const float* rays_d;
-    const float* near_planes;  // per ray, or null: near_plane for every ray
-    const float* far_planes;
-    float near_plane, far_plane;
-    OccGeom g;
-    const uint64_t* words;
-    const uint32_t* coarse;
-    const float* aabbs;
-    const float* t_sorted;  // null: one level, crossings computed in the kernel
-    const int64_t* t_indices;
-    const uint8_t* hits;
-    float step_size, cone_angle;
-    Workspace ws;
-    int64_t* totals;
-    int64_t* totals_host;
-};
-
 // RunSink pool of the march kernel: the lanes that close a run at the same time take their slots with one atomic
 struct PoolAppend {
     uint32_t* cursor;
@@ -1099,7 +1084,7 @@ struct PoolAppend {
 // One thread per ray, tiles of ws.tile_rays rays in ray order, the walk of march_generic.cuh.  A ray whose marching
 // variable stops advancing ends there, as in generic_traverse_kernel: the stuck count stays 0.
 template <bool kSingle>
-__global__ void __launch_bounds__(kMaxTileRays) march_cone_kernel(const ConeParams p)
+__global__ void __launch_bounds__(kMaxTileRays) march_cone_kernel(const MarchParams p)
 {
     __shared__ uint32_t s_cnt[kMaxTileRays];
     const int tid = threadIdx.x;
@@ -1145,15 +1130,11 @@ __global__ void __launch_bounds__(kMaxTileRays) march_cone_kernel(const ConePara
 // [tile base + samples of the tile's earlier rays + samples of the ray before the run] (the dependent loads of 32
 // runs in flight together), then the warp writes the runs one after the other, lane j sample j of each piece of 32
 // (march_generic.cuh, cone_expand_run: the same float operations in the same order), so that stores coalesce.
-__global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const Workspace ws, int32_t n_rays,
-                                                                     const int64_t* totals, float step_size,
-                                                                     float cone_angle, int64_t capacity,
-                                                                     int64_t* packed_info, int64_t* ray_indices,
-                                                                     float* t_starts, float* t_ends)
+__global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const SamplesParams p)
 {
     static_assert(kExpandLanes == 32, "one lane per sample of a piece");
-    write_packed_info(ws, n_rays, packed_info);
-    const int64_t n_runs = pool_runs(ws, totals);
+    write_packed_info(p.ws, p.n_rays, p.packed_info);
+    const int64_t n_runs = pool_runs(p.ws, p.totals);
     const int lane = threadIdx.x & 31;
     const int64_t warp0 = ((int64_t)blockIdx.x * kExpandThreads + threadIdx.x) >> 5;
     const int64_t n_warps = ((int64_t)gridDim.x * kExpandThreads) >> 5;
@@ -1163,7 +1144,7 @@ __global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const Works
         float my_first = 0.f;
         int64_t my_k0 = 0;
         if (q < n_runs) {
-            const uint4 a = load_run(ws, q, my_k0);
+            const uint4 a = load_run(p.ws, q, my_k0);
             my_ray = a.x;
             my_n = a.z;
             my_first = __uint_as_float(a.w);
@@ -1176,13 +1157,13 @@ __global__ void __launch_bounds__(kExpandThreads) expand_cone_kernel(const Works
             float t = __shfl_sync(0xffffffffu, my_first, i);
             for (uint32_t base = 0; base < n; base += 32) {
                 const uint32_t m = min(n - base, 32u);
-                const float ts = cone_advance(t, min((uint32_t)lane, m - 1u), cone_angle, step_size);
-                const float te = cone_next(ts, cone_angle, step_size);
+                const float ts = cone_advance(t, min((uint32_t)lane, m - 1u), p.cone_angle, p.step_size);
+                const float te = cone_next(ts, p.cone_angle, p.step_size);
                 const int64_t k = k0 + base + lane;
-                if ((uint32_t)lane < m && k < capacity) {
-                    ray_indices[k] = ray;
-                    t_starts[k] = ts;
-                    t_ends[k] = te;
+                if ((uint32_t)lane < m && k < p.capacity) {
+                    p.ray_indices[k] = ray;
+                    p.t_starts[k] = ts;
+                    p.t_ends[k] = te;
                 }
                 t = __shfl_sync(0xffffffffu, te, (int)m - 1);
             }
@@ -1286,27 +1267,6 @@ static void launch_march(const MarchParams& p, int tiles, int threads, cudaStrea
     march_kernel<kSingle, kSlots><<<tiles, threads, dyn, s>>>(p);
 }
 
-// The argument rules nfa_march and nfa_march_cone share.  True when there are rays to march; otherwise `status` is
-// what the call returns: an argument error or, with no rays, that of zeroing the totals (device and pinned mirror).
-static bool march_args_ok(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
-                          const float* far_planes, int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
-                          const uint64_t* words, const float* aabbs, bool have_sorted, float step_size,
-                          int64_t run_capacity, const void* workspace, int64_t* totals, int64_t* totals_host,
-                          cudaStream_t s, int32_t& status)
-{
-    if (n_rays < 0 || n_grids <= 0 || rx <= 0 || ry <= 0 || rz <= 0 || run_capacity < 0) status = NFA_ERR_ARG;
-    else if (run_capacity > (int64_t)UINT32_MAX || !(step_size > 0.0f)) status = NFA_ERR_UNSUPPORTED;
-    else if (!totals || (near_planes == nullptr) != (far_planes == nullptr)) status = NFA_ERR_ARG;
-    else if (n_rays == 0) {
-        if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
-        status = (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
-    } else if (!rays_o || !rays_d || !words || !aabbs || !workspace || (!have_sorted && n_grids != 1))
-        status = NFA_ERR_ARG;  // (nested levels need the sorted crossings)
-    else
-        return true;
-    return false;
-}
-
 // Expand grid for `threads` threads: at least one CTA, at most the 8 CTAs of kExpandThreads resident per SM.
 static inline int expand_grid(int64_t threads)
 {
@@ -1317,8 +1277,8 @@ static inline int expand_grid(int64_t threads)
 
 extern "C" {
 
-// measurement aid, not part of the product path: per-warp time stamps of the next nfa_march launches go to
-// `buffer` (8 x u64 per warp, n_tiles x 16 warps); null switches it off
+// measurement aid, not part of the product path: per-warp time stamps of the next constant-step nfa_march launches
+// (march_kernel) go to `buffer` (8 x u64 per warp, n_tiles x 16 warps); null switches it off
 void nfa_debug_set_march_trace(void* buffer) { g_march_trace = (unsigned long long*)buffer; }
 
 int32_t nfa_version(void) { return NFA_ABI_VERSION; }
@@ -1393,19 +1353,27 @@ int64_t nfa_march_workspace_bytes(int32_t n_rays, int64_t run_capacity)
 
 int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
                   const float* far_planes, float near_plane, float far_plane, int32_t n_grids, int32_t rx,
-                  int32_t ry, int32_t rz,
-                  const uint64_t* words, const int32_t* bounds, const float* aabbs,
-                  const float* t_sorted, const int64_t* t_indices, const uint8_t* hits, float step_size,
-                  int64_t run_capacity, void* workspace, int64_t* totals, int64_t* totals_host,
-                  float* terminate_planes, nfa_stream_t stream)
+                  int32_t ry, int32_t rz, const uint64_t* words, const uint32_t* coarse, const int32_t* bounds,
+                  const float* aabbs, const float* t_sorted, const int64_t* t_indices, const uint8_t* hits,
+                  float step_size, float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
+                  int64_t* totals_host, float* terminate_planes, nfa_stream_t stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
     const bool have_sorted = t_sorted && t_indices && hits;
-    int32_t status;
-    if (!march_args_ok(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, aabbs, have_sorted,
-                       step_size, run_capacity, workspace, totals, totals_host, s, status))
-        return status;
-    MarchParams p;
+    const bool cone = cone_angle > 0.0f;
+    // !(cone_angle >= 0): negative or NaN
+    if (n_rays < 0 || n_grids <= 0 || rx <= 0 || ry <= 0 || rz <= 0 || run_capacity < 0 || !(cone_angle >= 0.0f))
+        return NFA_ERR_ARG;
+    if (run_capacity > (int64_t)UINT32_MAX || !(step_size > 0.0f)) return NFA_ERR_UNSUPPORTED;
+    if (!totals || (near_planes == nullptr) != (far_planes == nullptr) || (cone && !coarse)) return NFA_ERR_ARG;
+    if (cone && terminate_planes) return NFA_ERR_UNSUPPORTED;  // the growing-step walk does not write them
+    if (n_rays == 0) {
+        if (totals_host) totals_host[0] = totals_host[1] = totals_host[2] = totals_host[3] = 0;
+        return (int32_t)cudaMemsetAsync(totals, 0, 4 * sizeof(int64_t), s);
+    }
+    if (!rays_o || !rays_d || !words || !aabbs || !workspace || (!have_sorted && n_grids != 1))
+        return NFA_ERR_ARG;  // (nested levels need the sorted crossings)
+    MarchParams p = {};  // zero: no lattice table, no trace
     p.n_rays = n_rays;
     p.rays_o = rays_o;
     p.rays_d = rays_d;
@@ -1415,15 +1383,25 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
     p.far_plane = far_plane;
     p.g = occ_geom(n_grids, rx, ry, rz);
     p.words = words;
+    p.coarse = coarse;
     p.bounds = bounds;
     p.aabbs = aabbs;
     p.t_sorted = have_sorted ? t_sorted : nullptr;
     p.t_indices = have_sorted ? t_indices : nullptr;
     p.hits = have_sorted ? hits : nullptr;
     p.step_size = step_size;
+    p.cone_angle = cone_angle;
+    p.ws = ws_view(workspace, n_rays, run_capacity);
+    p.totals = totals;
+    p.totals_host = totals_host;
+    p.terminate = terminate_planes;
+    const int tiles = p.ws.n_tiles, threads = p.ws.tile_rays;
+    if (cone) {  // growing step: no lattice, so no lattice table, and the trace covers march_kernel only
+        if (have_sorted) march_cone_kernel<false><<<tiles, threads, 0, s>>>(p);
+        else march_cone_kernel<true><<<tiles, threads, 0, s>>>(p);
+        return launch_status();
+    }
     p.trace = g_march_trace;
-    p.lat_table.n = 0;
-    p.lat_table.e0 = 0;
     if (near_planes == nullptr && step_size > 0.f) {  // the climb from the near plane, once per (step, near plane)
         static thread_local LatTable cached;
         static thread_local float cached_dt = 0.f, cached_near = 0.f;
@@ -1436,11 +1414,6 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
         }
         p.lat_table = cached;
     }
-    p.ws = ws_view(workspace, n_rays, run_capacity);
-    p.totals = totals;
-    p.totals_host = totals_host;
-    p.terminate = terminate_planes;
-    const int tiles = p.ws.n_tiles, threads = p.ws.tile_rays;
     // one wave (every tile resident at once, at most two per SM): room for twice the descriptor slots
     const bool wide = tiles <= 2 * kNumSMs && threads >= 224;
     if (!have_sorted) {
@@ -1454,21 +1427,27 @@ int32_t nfa_march(int32_t n_rays, const float* rays_o, const float* rays_d, cons
 }
 
 int32_t nfa_expand_samples(int32_t n_rays, int64_t run_capacity, const void* workspace, const int64_t* totals,
-                           float step_size, int64_t capacity, int64_t* packed_info, int64_t* ray_indices,
-                           float* t_starts, float* t_ends, nfa_stream_t stream)
+                           float step_size, float cone_angle, int64_t capacity, int64_t* packed_info,
+                           int64_t* ray_indices, float* t_starts, float* t_ends, nfa_stream_t stream)
 {
-    if (n_rays < 0 || capacity < 0 || run_capacity < 0) return NFA_ERR_ARG;
+    // !(cone_angle >= 0): negative or NaN
+    if (n_rays < 0 || capacity < 0 || run_capacity < 0 || !(cone_angle >= 0.0f)) return NFA_ERR_ARG;
     if (n_rays == 0) return NFA_OK;
     if (!workspace || !packed_info || !totals) return NFA_ERR_ARG;
     if (capacity > 0 && (!ray_indices || !t_starts || !t_ends)) return NFA_ERR_ARG;
     if ((((uintptr_t)packed_info) & 15u) != 0) return NFA_ERR_ARG;
     const SamplesParams p = {ws_view(const_cast<void*>(workspace), n_rays, run_capacity), n_rays, totals, step_size,
-                             capacity, packed_info, ray_indices, t_starts, t_ends};
-    // a warp per run, and a thread per ray for packed_info (written even when nothing is expanded)
-    const int grid = expand_grid(32 * run_capacity > n_rays ? 32 * run_capacity : n_rays);
-    const bool vec = (((uintptr_t)ray_indices | (uintptr_t)t_starts | (uintptr_t)t_ends) & 15u) == 0;
+                             cone_angle, capacity, packed_info, ray_indices, t_starts, t_ends};
     const cudaStream_t s = (cudaStream_t)stream;
-    (vec ? expand_samples_kernel<true> : expand_samples_kernel<false>)<<<grid, kExpandThreads, 0, s>>>(p);
+    if (cone_angle > 0.0f) {
+        // a lane per run, and a thread per ray for packed_info
+        expand_cone_kernel<<<expand_grid(run_capacity > n_rays ? run_capacity : n_rays), kExpandThreads, 0, s>>>(p);
+    } else {
+        // a warp per run, and a thread per ray for packed_info (written even when nothing is expanded)
+        const int grid = expand_grid(32 * run_capacity > n_rays ? 32 * run_capacity : n_rays);
+        const bool vec = (((uintptr_t)ray_indices | (uintptr_t)t_starts | (uintptr_t)t_ends) & 15u) == 0;
+        (vec ? expand_samples_kernel<true> : expand_samples_kernel<false>)<<<grid, kExpandThreads, 0, s>>>(p);
+    }
     return launch_status();
 }
 
@@ -1493,63 +1472,6 @@ int32_t nfa_expand_intervals(int32_t n_rays, int64_t run_capacity, const void* w
                                    iv_packed_info, iv_ray_indices, iv_vals, iv_is_left, iv_is_right, edge_capacity};
         expand_intervals_kernel<<<expand_grid(32 * run_capacity), kExpandThreads, 0, s>>>(p);
     }
-    return launch_status();
-}
-
-int32_t nfa_march_cone(int32_t n_rays, const float* rays_o, const float* rays_d, const float* near_planes,
-                       const float* far_planes, float near_plane, float far_plane, int32_t n_grids, int32_t rx,
-                       int32_t ry, int32_t rz, const uint64_t* words, const uint32_t* coarse, const float* aabbs,
-                       const float* t_sorted, const int64_t* t_indices, const uint8_t* hits, float step_size,
-                       float cone_angle, int64_t run_capacity, void* workspace, int64_t* totals,
-                       int64_t* totals_host, nfa_stream_t stream)
-{
-    cudaStream_t s = (cudaStream_t)stream;
-    const bool have_sorted = t_sorted && t_indices && hits;
-    int32_t status;
-    if (!march_args_ok(n_rays, rays_o, rays_d, near_planes, far_planes, n_grids, rx, ry, rz, words, aabbs, have_sorted,
-                       step_size, run_capacity, workspace, totals, totals_host, s, status))
-        return status;
-    if (!coarse) return NFA_ERR_ARG;
-    ConeParams p;
-    p.n_rays = n_rays;
-    p.rays_o = rays_o;
-    p.rays_d = rays_d;
-    p.near_planes = near_planes;
-    p.far_planes = far_planes;
-    p.near_plane = near_plane;
-    p.far_plane = far_plane;
-    p.g = occ_geom(n_grids, rx, ry, rz);
-    p.words = words;
-    p.coarse = coarse;
-    p.aabbs = aabbs;
-    p.t_sorted = have_sorted ? t_sorted : nullptr;
-    p.t_indices = have_sorted ? t_indices : nullptr;
-    p.hits = have_sorted ? hits : nullptr;
-    p.step_size = step_size;
-    p.cone_angle = cone_angle;
-    p.ws = ws_view(workspace, n_rays, run_capacity);
-    p.totals = totals;
-    p.totals_host = totals_host;
-    if (have_sorted) march_cone_kernel<false><<<p.ws.n_tiles, p.ws.tile_rays, 0, s>>>(p);
-    else march_cone_kernel<true><<<p.ws.n_tiles, p.ws.tile_rays, 0, s>>>(p);
-    return launch_status();
-}
-
-int32_t nfa_expand_cone_samples(int32_t n_rays, int64_t run_capacity, const void* workspace, const int64_t* totals,
-                                float step_size, float cone_angle, int64_t capacity, int64_t* packed_info,
-                                int64_t* ray_indices, float* t_starts, float* t_ends, nfa_stream_t stream)
-{
-    if (n_rays < 0 || capacity < 0 || run_capacity < 0) return NFA_ERR_ARG;
-    if (n_rays == 0) return NFA_OK;
-    if (!workspace || !packed_info || !totals) return NFA_ERR_ARG;
-    if (capacity > 0 && (!ray_indices || !t_starts || !t_ends)) return NFA_ERR_ARG;
-    if ((((uintptr_t)packed_info) & 15u) != 0) return NFA_ERR_ARG;
-    const Workspace ws = ws_view(const_cast<void*>(workspace), n_rays, run_capacity);
-    // a lane per run, and a thread per ray for packed_info
-    const int grid = expand_grid(run_capacity > n_rays ? run_capacity : n_rays);
-    expand_cone_kernel<<<grid, kExpandThreads, 0, (cudaStream_t)stream>>>(ws, n_rays, totals, step_size, cone_angle,
-                                                                          capacity, packed_info, ray_indices, t_starts,
-                                                                          t_ends);
     return launch_status();
 }
 

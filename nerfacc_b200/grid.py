@@ -113,6 +113,19 @@ def _packed_grid(binaries: Tensor) -> _OccPack:
     return pack
 
 
+def _sorted_crossings(rays_o: Tensor, rays_d: Tensor, aabbs: Tensor, n_grids: int):
+    """(t_sorted, t_indices, hits): every ray's crossings of the `n_grids` nested boxes, ascending
+    (reference grid.py:156-162)."""
+    device, n_rays = rays_o.device, rays_o.shape[0]
+    t_sorted = torch.empty((n_rays, 2 * n_grids), dtype=torch.float32, device=device)
+    t_indices = torch.empty((n_rays, 2 * n_grids), dtype=torch.int64, device=device)
+    hits = torch.empty((n_rays, n_grids), dtype=torch.bool, device=device)
+    if n_rays > 0:
+        _lib.call("nfa_intersect_sorted", device, n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), n_grids,
+                  _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices), _lib.ptr(hits))
+    return t_sorted, t_indices, hits
+
+
 class _MarchScratch:
     """Reusable march workspace (counts, tile sums, run pool) + pinned read-back slot of one (device, stream).
 
@@ -179,8 +192,8 @@ class _MarchJob:
     the hint (or the run pool) and returns the result.  `near_planes` / `far_planes` may both be None: every ray
     then uses the scalars.  The job keeps its inputs alive and owns its workspace until `finish()`.
 
-    `cone_angle == 0`: constant step (nfa_march / nfa_expand_*).  `cone_angle > 0`: the step grows with the distance
-    (nfa_march_cone / nfa_expand_cone_samples), samples only -- no interval form, no terminate planes.
+    `cone_angle == 0`: constant step.  `cone_angle > 0`: the step grows with the distance, samples only -- no interval
+    form, no terminate planes.
     """
 
     def __init__(self, rays_o: Tensor, rays_d: Tensor, binaries: Tensor, aabbs: Tensor, near_planes: Optional[Tensor],
@@ -197,12 +210,7 @@ class _MarchJob:
         n_grids = self.shape[0]
         self.occ = _packed_grid(binaries)
         if n_grids > 1 and t_sorted is None:
-            t_sorted = torch.empty((n_rays, 2 * n_grids), dtype=torch.float32, device=device)
-            t_indices = torch.empty((n_rays, 2 * n_grids), dtype=torch.int64, device=device)
-            hits = torch.empty((n_rays, n_grids), dtype=torch.bool, device=device)
-            if n_rays > 0:
-                _lib.call("nfa_intersect_sorted", device, n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), n_grids,
-                          _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices), _lib.ptr(hits))
+            t_sorted, t_indices, hits = _sorted_crossings(rays_o, rays_d, aabbs, n_grids)
         self.inputs = (rays_o, rays_d, aabbs, near_planes, far_planes, t_sorted, t_indices, hits)
         self.planes = (float(near_plane), float(far_plane))
         self.step_size = float(step_size)
@@ -221,18 +229,11 @@ class _MarchJob:
         rays_o, rays_d, aabbs, near_planes, far_planes, t_sorted, t_indices, hits = self.inputs
         n_grids, rx, ry, rz = self.shape
         sc, occ = self.sc, self.occ
-        if self.cone_angle > 0.0:
-            _lib.call("nfa_march_cone", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d),
-                      _lib.ptr(near_planes), _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz,
-                      _lib.ptr(occ.words), _lib.ptr(occ.coarse), _lib.ptr(aabbs), _lib.ptr(t_sorted),
-                      _lib.ptr(t_indices), _lib.ptr(hits), self.step_size, self.cone_angle, sc.run_capacity,
-                      _lib.ptr(sc.workspace), _lib.ptr(sc.totals_dev), _lib.ptr(sc.totals_host))
-        else:
-            _lib.call("nfa_march", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(near_planes),
-                      _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz, _lib.ptr(occ.words),
-                      _lib.ptr(occ.bounds), _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices),
-                      _lib.ptr(hits), self.step_size, sc.run_capacity, _lib.ptr(sc.workspace), _lib.ptr(sc.totals_dev),
-                      _lib.ptr(sc.totals_host), _lib.ptr(self.term))
+        _lib.call("nfa_march", self.device, self.n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(near_planes),
+                  _lib.ptr(far_planes), self.planes[0], self.planes[1], n_grids, rx, ry, rz, _lib.ptr(occ.words),
+                  _lib.ptr(occ.coarse), _lib.ptr(occ.bounds), _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices),
+                  _lib.ptr(hits), self.step_size, self.cone_angle, sc.run_capacity, _lib.ptr(sc.workspace),
+                  _lib.ptr(sc.totals_dev), _lib.ptr(sc.totals_host), _lib.ptr(self.term))
         # on the stream (of THIS device) the march was launched on: the default `record()` would use the current
         # device's stream and the totals could be read before they are written
         sc.event.record(torch.cuda.current_stream(self.device))
@@ -256,14 +257,9 @@ class _MarchJob:
         ri = torch.empty(cap, dtype=torch.int64, device=device)
         ts = torch.empty(cap, dtype=torch.float32, device=device)
         te = torch.empty(cap, dtype=torch.float32, device=device)
-        if self.cone_angle > 0.0:
-            _lib.call("nfa_expand_cone_samples", device, self.n_rays, sc.run_capacity, _lib.ptr(sc.workspace),
-                      _lib.ptr(sc.totals_dev), self.step_size, self.cone_angle, cap, _lib.ptr(self.packed_info),
-                      _lib.ptr(ri), _lib.ptr(ts), _lib.ptr(te))
-        else:
-            _lib.call("nfa_expand_samples", device, self.n_rays, sc.run_capacity, _lib.ptr(sc.workspace),
-                      _lib.ptr(sc.totals_dev), self.step_size, cap, _lib.ptr(self.packed_info), _lib.ptr(ri),
-                      _lib.ptr(ts), _lib.ptr(te))
+        _lib.call("nfa_expand_samples", device, self.n_rays, sc.run_capacity, _lib.ptr(sc.workspace),
+                  _lib.ptr(sc.totals_dev), self.step_size, self.cone_angle, cap, _lib.ptr(self.packed_info),
+                  _lib.ptr(ri), _lib.ptr(ts), _lib.ptr(te))
         return ri, ts, te
 
     def begin(self) -> "_MarchJob":
@@ -388,12 +384,7 @@ def _traverse_generic(rays_o, rays_d, binaries, aabbs, near_planes, far_planes, 
     n_grids, rx, ry, rz = (int(s) for s in binaries.shape)
     occ = _packed_grid(binaries)
     if t_sorted is None:
-        t_sorted = torch.empty((n_rays, 2 * n_grids), dtype=torch.float32, device=device)
-        t_indices = torch.empty((n_rays, 2 * n_grids), dtype=torch.int64, device=device)
-        hits = torch.empty((n_rays, n_grids), dtype=torch.bool, device=device)
-        if n_rays > 0:
-            _lib.call("nfa_intersect_sorted", device, n_rays, _lib.ptr(rays_o), _lib.ptr(rays_d), n_grids,
-                      _lib.ptr(aabbs), _lib.ptr(t_sorted), _lib.ptr(t_indices), _lib.ptr(hits))
+        t_sorted, t_indices, hits = _sorted_crossings(rays_o, rays_d, aabbs, n_grids)
     if t_indices.dtype != torch.int64:
         t_indices = t_indices.to(torch.int64)
     if hits.dtype != torch.bool:

@@ -1,6 +1,6 @@
-"""Growing-step sampling (cone_angle > 0) on one GPU: the route through nfa_march_cone / nfa_expand_cone_samples
-against the traverse_grids route it replaced, and against the reference CUDA build, on the 360-like case of
-oracle/gen_golden_cone_gpu.py (65 536 rays, 4 x 128^3 levels, step 1e-3, cone 0.004, near 0.2).
+"""Growing-step sampling (cone_angle > 0) on one GPU: the route through nfa_march / nfa_expand_samples with
+cone_angle > 0 against the traverse_grids route it replaced, and against the reference CUDA build, on the 360-like
+case of oracle/gen_golden_cone_gpu.py (65 536 rays, 4 x 128^3 levels, step 1e-3, cone 0.004, near 0.2).
 
     python scripts/cone_probe.py [--iters N] [--out FILE]   # prints JSON; --out: the result also as a JSON file
 
@@ -8,7 +8,8 @@ oracle/gen_golden_cone_gpu.py (65 536 rays, 4 x 128^3 levels, step 1e-3, cone 0.
   process after warm-up, without and with the visibility filter (sigma_fn, alpha_thre 1e-2); median and spread.
 - the reference CUDA build (oracle/_ref) on the same inputs, in a child process (its `nerfacc` package and this
   repository's must not meet in one interpreter).
-- walk and expand kernel times from CUDA events over repeated launches, the sample count N, and the expand's
+- walk and expand kernel times from CUDA events over repeated launches through the sampling job's own launch
+  methods (_MarchJob._launch_march / _expand_samples, the calls sampling() makes), the sample count N, and the expand's
   16 B/sample (int64 ray index + two float32) over its time next to a fill_ of the same number of bytes.
 """
 import argparse
@@ -93,8 +94,7 @@ def main():
     if args.reference:
         return reference(args.iters)
     import nerfacc_b200 as nfa
-    from nerfacc_b200 import _lib
-    from nerfacc_b200.grid import _packed_grid, traverse_grids
+    from nerfacc_b200.grid import _MarchJob, traverse_grids
     dev = torch.device("cuda:0")
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
                        capture_output=True, text=True)
@@ -125,47 +125,22 @@ def main():
     n = int(est.sampling(o, d, **kw)[0].numel())
     n_kept = int(est.sampling(o, d, **kw, **filt)[0].numel())
 
-    # kernels alone, into a workspace of our own
-    lib = _lib.load()
-    R, G = o.shape[0], c["levels"]
-    occ = _packed_grid(est.binaries)
-    aab = est.aabbs.contiguous().float()
-    t_sorted = torch.empty((R, 2 * G), dtype=torch.float32, device=dev)
-    t_indices = torch.empty((R, 2 * G), dtype=torch.int64, device=dev)
-    hits = torch.empty((R, G), dtype=torch.bool, device=dev)
-    _lib.call("nfa_intersect_sorted", dev, R, o.data_ptr(), d.data_ptr(), G, aab.data_ptr(), t_sorted.data_ptr(),
-              t_indices.data_ptr(), hits.data_ptr())
-    cap = 4 * R + 1024
-    ws = torch.zeros(lib.nfa_march_workspace_bytes(R, cap), dtype=torch.uint8, device=dev)
-    tot = torch.zeros(4, dtype=torch.int64, device=dev)
-    rx, ry, rz = (int(v) for v in est.binaries.shape[1:])
-
-    def walk():
-        _lib.call("nfa_march_cone", dev, R, o.data_ptr(), d.data_ptr(), None, None, c["near"], 1e10, G, rx, ry, rz,
-                  occ.words.data_ptr(), occ.coarse.data_ptr(), aab.data_ptr(), t_sorted.data_ptr(),
-                  t_indices.data_ptr(), hits.data_ptr(), c["step"], c["cone"], cap, ws.data_ptr(), tot.data_ptr(), None)
-
-    walk()
-    torch.cuda.synchronize()
-    if int(tot[1]) > cap:  # run pool too small: march again with room for every run
-        cap = int(tot[1]) + 1024
-        ws = torch.zeros(lib.nfa_march_workspace_bytes(R, cap), dtype=torch.uint8, device=dev)
-        walk()
-        torch.cuda.synchronize()
-    n_k, runs = int(tot[0]), int(tot[1])
-    assert n_k == n and runs <= cap, (n_k, n, runs, cap)
-    pi = torch.empty((R, 2), dtype=torch.int64, device=dev)
-    ri = torch.empty(n, dtype=torch.int64, device=dev)
-    ts = torch.empty(n, dtype=torch.float32, device=dev)
-    te = torch.empty(n, dtype=torch.float32, device=dev)
-
-    def expand():
-        _lib.call("nfa_expand_cone_samples", dev, R, cap, ws.data_ptr(), tot.data_ptr(), c["step"], c["cone"], n,
-                  pi.data_ptr(), ri.data_ptr(), ts.data_ptr(), te.data_ptr())
+    # kernels alone, launched the way sampling() launches them (as bench.py times the constant-step ones)
+    job = _MarchJob(o, d, est.binaries, est.aabbs, None, None, c["step"], None, None, None, want_intervals=False,
+                    want_terminate=False, near_plane=c["near"], far_plane=1e10, cone_angle=c["cone"])
+    job._launch_march()
+    n_k, runs = job._read_totals()
+    if runs > job.sc.run_capacity:  # run pool too small: march again with room for every run
+        job.sc.reserve(o.shape[0], runs + 1024)
+        job._launch_march()
+        n_k, runs = job._read_totals()
+    assert n_k == n, (n_k, n)
 
     fill_buf = torch.empty(16 * n, dtype=torch.uint8, device=dev)
     it = 200
-    t_walk, t_expand = _events(walk, it), _events(expand, it)
+    t_walk, t_expand = _events(job._launch_march, it), _events(lambda: job._expand_samples(n), it)
+    job.sc.busy = False
+    job.sc = None
     t_fill = _events(lambda: fill_buf.fill_(1), it)
     kernels = dict(n_samples=n, n_runs=runs, samples_per_run=n / max(runs, 1), walk_ms=t_walk, expand_ms=t_expand,
                    expand_GBps=16 * n / (t_expand * 1e-3) / 1e9, fill_same_bytes_ms=t_fill,

@@ -68,6 +68,22 @@ def test_argument_errors_do_not_need_a_gpu():
     assert lib.nfa_intersect_sorted(1, None, None, 64, None, None, None, None, None) == -2  # > 32 boxes: unsupported
     assert lib.nfa_march_workspace_bytes(-5, 10) == 0
 
+    # cone_angle rules of nfa_march / nfa_expand_samples: rejected before any pointer is read, so every other
+    # pointer may be a dummy (non-null, 16-byte aligned) address
+    P = 1 << 20
+
+    def march(cone_angle, coarse=P, terminate_planes=None):
+        return lib.nfa_march(64, P, P, None, None, 0.0, 1e10, 1, 32, 32, 32, P, coarse, P, P, None, None, None, 1e-3,
+                             cone_angle, 1024, P, P, None, terminate_planes, None)
+
+    def expand(cone_angle):
+        return lib.nfa_expand_samples(64, 1024, P, P, 1e-3, cone_angle, 4096, P, P, P, P, None)
+
+    for bad in (-0.004, float("nan")):
+        assert march(bad) == -1 and expand(bad) == -1
+    assert march(0.004, coarse=None) == -1
+    assert march(0.004, terminate_planes=P) == -2  # the growing-step walk writes no terminate planes
+
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
     from nerfacc_b200 import _lib

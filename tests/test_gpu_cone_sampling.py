@@ -1,7 +1,7 @@
-"""OccGridEstimator.sampling with growing steps (cone_angle > 0) on the GPU: nfa_march_cone + nfa_expand_cone_samples
-behind sampling_begin / sampling_end.  Bit-exact against the CPU oracle, against the traverse_grids route this path
-replaced (edge/flag form + mask-selects), and against the reference CUDA build (tests/golden/ref_live_cone360.npz,
-oracle/gen_golden_cone_gpu.py)."""
+"""OccGridEstimator.sampling with growing steps (cone_angle > 0) on the GPU: nfa_march + nfa_expand_samples with
+cone_angle > 0 (march_cone_kernel, expand_cone_kernel) behind sampling_begin / sampling_end.  Bit-exact against the
+CPU oracle, against the traverse_grids route this path replaced (edge/flag form + mask-selects), and against the
+reference CUDA build (tests/golden/ref_live_cone360.npz, oracle/gen_golden_cone_gpu.py)."""
 import numpy as np
 import pytest
 import torch

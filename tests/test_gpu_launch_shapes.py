@@ -410,7 +410,7 @@ GUARD = 256
 F_SENT, I_SENT, B_SENT = -1234.5, -7, 0xAB
 
 
-def _march_abi(name):
+def _march_abi(name, cone_angle=0.0):
     """One nfa_march of a scene's distinct rays into a workspace of our own; returns what the expand calls need."""
     from nerfacc_b200 import _lib, grid as _grid
     lib = _lib.load()
@@ -431,11 +431,12 @@ def _march_abi(name):
     ws = torch.zeros(lib.nfa_march_workspace_bytes(R, cap), dtype=torch.uint8, device=dev)
     tot = torch.zeros(4, dtype=torch.int64, device=dev)
     _lib.call("nfa_march", device, R, o.data_ptr(), d.data_ptr(), None, None, 0.0, far, G, rx, ry, rz,
-              occ.words.data_ptr(), occ.bounds.data_ptr(), a.data_ptr(), _lib.ptr(tsrt), _lib.ptr(tidx), _lib.ptr(hits),
-              step, cap, ws.data_ptr(), tot.data_ptr(), None, None)
+              occ.words.data_ptr(), occ.coarse.data_ptr(), occ.bounds.data_ptr(), a.data_ptr(), _lib.ptr(tsrt),
+              _lib.ptr(tidx), _lib.ptr(hits), step, cone_angle, cap, ws.data_ptr(), tot.data_ptr(), None, None)
     n, runs, _, stuck = (int(v) for v in N(tot))
     assert stuck == 0 and 0 < runs <= cap
-    return dict(R=R, cap=cap, ws=ws, tot=tot, step=step, n=n, runs=runs, keep=(occ, o, d, a, tsrt, tidx, hits))
+    return dict(R=R, cap=cap, ws=ws, tot=tot, step=step, cone=cone_angle, n=n, runs=runs,
+                keep=(occ, o, d, a, tsrt, tidx, hits))
 
 
 def _expand_samples(m, capacity, offsets=(0, 0), run_capacity=None):
@@ -451,22 +452,26 @@ def _expand_samples(m, capacity, offsets=(0, 0), run_capacity=None):
     ts, te, ri = ts_buf[fo:], te_buf[fo:], ri_buf[io:]
     run_capacity = m["cap"] if run_capacity is None else run_capacity
     _lib.call("nfa_expand_samples", torch.device(dev), m["R"], run_capacity, m["ws"].data_ptr(), m["tot"].data_ptr(),
-              m["step"], capacity, pi.data_ptr(), ri.data_ptr(), ts.data_ptr(), te.data_ptr())
+              m["step"], m["cone"], capacity, pi.data_ptr(), ri.data_ptr(), ts.data_ptr(), te.data_ptr())
     torch.cuda.synchronize()
     return N(pi), (N(ri_buf), N(ts_buf), N(te_buf)), (N(ri), N(ts), N(te))
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("cone_angle", [0.0, 0.004], ids=["const", "cone"])
 @pytest.mark.parametrize("name", ["frag1", "comb4"])
-def test_expand_samples_clipped_and_unaligned(orc, name):
+def test_expand_samples_clipped_and_unaligned(orc, name, cone_angle):
     """nfa_expand_samples with capacity n - k (the speculative call whose batch outgrew the hint): the first
     `capacity` elements are the full result, nothing at or past `capacity` is written, packed_info is complete.
     Capacity 0 (k = n) and an empty run pool (run_capacity 0) write packed_info and nothing else.  With outputs
-    4 / 8 bytes off 16-byte alignment (element-wise stores) the result is byte-identical."""
+    4 / 8 bytes off 16-byte alignment (element-wise stores) the result is byte-identical.  Both kernels the call
+    chooses from: constant step (expand_samples_kernel) and growing step (cone_angle > 0, expand_cone_kernel; every
+    step of these two scenes grows at cone 0.004)."""
     bins, aabbs, ro, rd, step, far = scene(name)
-    m = _march_abi(name)
+    m = _march_abi(name, cone_angle)
     n = m["n"]
-    o_ri, o_ts, o_te, o_pi = orc.occgrid_sampling(ro, rd, bins, aabbs, render_step_size=step, far_plane=far)
+    o_ri, o_ts, o_te, o_pi = orc.occgrid_sampling(ro, rd, bins, aabbs, render_step_size=step, far_plane=far,
+                                                  cone_angle=cone_angle)
     pi, _, (ri, ts, te) = _expand_samples(m, n)
     ri, ts, te = ri[:n], ts[:n], te[:n]
     np.testing.assert_array_equal(pi, o_pi)
@@ -489,7 +494,7 @@ def test_expand_samples_clipped_and_unaligned(orc, name):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", ["frag1", "comb4"])
+@pytest.mark.parametrize("name", SCENES)
 def test_expand_intervals_clipped(orc, name):
     """nfa_expand_intervals with edge_capacity / sample_capacity below the totals: the kept prefix of every array is
     the full result, nothing past a capacity is written, both packed_info arrays are complete; the full result is

@@ -28,7 +28,7 @@ extern "C" {
 #define NFA_ERR_ARG (-1)         /* null pointer / negative size / inconsistent sizes */
 #define NFA_ERR_UNSUPPORTED (-2) /* valid request outside what this build implements */
 
-#define NFA_ABI_VERSION 14
+#define NFA_ABI_VERSION 15
 
 typedef void* nfa_stream_t; /* cudaStream_t */
 
@@ -323,6 +323,51 @@ int32_t nfa_visibility_compact(int32_t n_rays, int64_t n_samples, const int64_t*
                                int32_t from_alpha, float early_stop_eps, float alpha_thre, void* workspace,
                                int64_t* new_packed_info, int64_t* out_ray_indices, float* out_t_starts,
                                float* out_t_ends, int64_t* total_dev, int64_t* total_host, nfa_stream_t stream);
+
+/* ----------------------------------------------------------------------- */
+/* Early-terminated test-time rendering (OccGridEstimator.render_test)      */
+/* ----------------------------------------------------------------------- */
+
+/* replaces: the test-mode rendering loop of nerfacc's examples (examples/utils.py:267-439): per round
+ *   traverse_grids(traverse_steps_limit, over_allocate, rays_mask, t_sorted, t_indices, hits), three boolean
+ *   mask-selects, render_weight_from_density(prefix_trans = 1 - opacity), the optional alpha_thre compaction, three
+ *   accumulate_along_rays_ and the new ray mask; then the background blend and depth normalisation.
+ * The workspace (nfa_render_test_workspace_bytes; 16-byte aligned, zeroed once when allocated, left reusable by every
+ *   call) holds the live-ray lists, every ray's near plane, the round's fixed-stride samples and the scans; it is
+ *   owned by one stream.  min_samples: 1 (cone_angle == 0) or 4.  Per call:
+ *   begin      every ray live, near planes = near_plane, kept-sample count 0.
+ *   march      round `round` (0, 1, ...): n_alive from the device (R, or what the previous composite left),
+ *              n_samples = max(min(R / n_alive, 64), min_samples), every live ray marched with that step limit
+ *              (t_sorted / t_indices / hits: nfa_intersect_sorted), its terminate plane kept as its next near plane;
+ *              status_host (pinned, [4]) = {n_alive, n_samples, samples of the round, kept samples of the earlier
+ *              rounds}, written when the kernel ends.  n_alive == 0: nothing was marched, the loop is over.
+ *              step_size <= 0 is NFA_ERR_UNSUPPORTED.
+ *   expand     the round's samples in ray order (the field's inputs); n_alive / n_samples from status_host.
+ *   composite  the field's float32 rgbs [n_total, 3] and sigmas [n_total] onto the running colors [R, 3], opacities
+ *              [R] and depths [R] (zero before round 0): weights from all the round's samples, alpha_thre > 0 drops
+ *              samples with alpha < alpha_thre from the sums only; a ray stays live while opacity <= opacity_thre
+ *              (1 - early_stop_eps) and it got n_samples samples.  Deterministic: no atomics on the outputs.
+ *   finish     colors += bkgd (1 - opacity) when bkgd [3] is given, depths /= max(opacity, FLT_EPSILON); with
+ *              status_host, status_host[3] = kept samples of all rounds. */
+int64_t nfa_render_test_workspace_bytes(int32_t n_rays, int32_t min_samples);
+int32_t nfa_render_test_begin(int32_t n_rays, int32_t min_samples, float near_plane, void* workspace,
+                              nfa_stream_t stream);
+int32_t nfa_render_test_march(int32_t n_rays, int32_t min_samples, int32_t round, const float* rays_o,
+                              const float* rays_d, float far_plane, int32_t n_grids, int32_t rx, int32_t ry, int32_t rz,
+                              const uint64_t* words, const uint32_t* coarse, const float* aabbs, const float* t_sorted,
+                              const int64_t* t_indices, const uint8_t* hits, float step_size, float cone_angle,
+                              void* workspace, int64_t* status_host, nfa_stream_t stream);
+int32_t nfa_render_test_expand(int32_t n_rays, int32_t min_samples, int32_t round, int32_t n_alive, int32_t n_samples,
+                               const void* workspace, int64_t* ray_indices, float* t_starts, float* t_ends,
+                               nfa_stream_t stream);
+int32_t nfa_render_test_composite(int32_t n_rays, int32_t min_samples, int32_t round, int32_t n_alive,
+                                  int32_t n_samples, int64_t n_total, void* workspace, const float* t_starts,
+                                  const float* t_ends, const float* rgbs, const float* sigmas, float alpha_thre,
+                                  float opacity_thre, float* colors, float* opacities, float* depths,
+                                  nfa_stream_t stream);
+int32_t nfa_render_test_finish(int32_t n_rays, int32_t min_samples, const void* workspace, const float* bkgd,
+                               float* colors, const float* opacities, float* depths, int64_t* status_host,
+                               nfa_stream_t stream);
 
 /* ----------------------------------------------------------------------- */
 /* PDF: importance sampling and per-ray searchsorted                        */

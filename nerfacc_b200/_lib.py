@@ -57,7 +57,14 @@ SIGNATURES = {
     "nfa_visibility_workspace_bytes": (_c_i64, [_c_i32, _c_i64]),
     "nfa_visibility_compact": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_i32, _c_f32, _c_f32]
                                + [_c_ptr] * 8),
-    "nfa_importance_sampling": (_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_i64, _c_i64,
+    "nfa_render_test_workspace_bytes": (_c_i64, [_c_i32, _c_i32]),
+    "nfa_render_test_begin": (_c_i32, [_c_i32, _c_i32, _c_f32, _c_ptr, _c_ptr]),
+    "nfa_render_test_march": (_c_i32, [_c_i32, _c_i32, _c_i32, _c_ptr, _c_ptr, _c_f32, _c_i32, _c_i32, _c_i32, _c_i32]
+                              + [_c_ptr] * 6 + [_c_f32, _c_f32, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_render_test_expand": (_c_i32, [_c_i32] * 5 + [_c_ptr] * 5),
+    "nfa_render_test_composite": (_c_i32, [_c_i32] * 5 + [_c_i64] + [_c_ptr] * 5 + [_c_f32, _c_f32] + [_c_ptr] * 4),
+    "nfa_render_test_finish": (_c_i32, [_c_i32, _c_i32] + [_c_ptr] * 7),
+    "nfa_importance_sampling":(_c_i32, [_c_i32, _c_ptr, _c_ptr, _c_ptr, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_i64, _c_i64,
                                          _c_i32, C.c_uint64, C.c_uint64] + [_c_ptr] * 8 + [_c_f32, _c_f32, _c_i32,
                                                                                           _c_ptr]),
     "nfa_searchsorted": (_c_i32, [_c_i64, _c_ptr, _c_ptr, _c_ptr, _c_i32, _c_i64, _c_ptr, _c_ptr, _c_i64, _c_ptr,
@@ -79,7 +86,7 @@ SIGNATURES = {
     "nfa_unpack_masked": (_c_i32, [_c_i32, _c_i64, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_ptr]),
 }
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 _lib = None
 launches = 0  # number of native kernel-launching calls made through this module (bench.py reports it)

@@ -7,6 +7,7 @@
 // fills at the scanned offsets (or one pass into fixed-stride slots when over-allocating).
 // The same walk with a run sink (RunSink) feeds nfa_march / nfa_expand_samples with cone_angle > 0, the
 // growing-step sampling path: runs instead of samples, one pass, replayed by the expand kernel.
+// With a sample sink (SampleSink) it is the round march of render_test.cu: fixed-stride samples of the live rays.
 // Reuses the DDA set-up, slab test, occupancy words and crossing iterators of march.cuh.
 // Host+device so that tests/host_sim can check it against the oracle on the CPU.
 #pragma once
@@ -139,6 +140,25 @@ NFA_HD void generic_emit(RunSink<Pool>& o, float t_last, float t_next, bool cont
     o.n_samples += 1;
 }
 
+// Sample sink (render_test.cu, OccGridEstimator.render_test): sample j of the ray as (t_starts, t_ends) at slot
+// base + j of two fixed-stride arrays.  t_start is t_last: an emission with `continuous` set starts where the previous
+// one ended, so this is the interval form's vals[is_left] / vals[is_right] pair without the edges.  The caller's
+// step limit bounds j.
+struct SampleSink {
+    float* t_starts;
+    float* t_ends;
+    int64_t base;
+    int64_t n_samples;  // samples of the ray so far (generic_march_ray's step limit reads it)
+};
+
+NFA_HD void generic_emit(SampleSink& o, float t_last, float t_next, bool continuous)
+{
+    (void)continuous;
+    o.t_starts[o.base + o.n_samples] = t_last;
+    o.t_ends[o.base + o.n_samples] = t_next;
+    o.n_samples += 1;
+}
+
 // The end of a sample that starts at t inside a run (reference grid.cu:215,259 with step_size > 0).
 NFA_HD float cone_next(float t, float cone, float step) { return f_add(t, step_length(t, cone, step)); }
 
@@ -176,7 +196,7 @@ NFA_HD void cone_expand_run(float t_first, uint32_t n, float cone, float step, i
     }
 }
 
-// March one ray into the sink `out` (GenericOut or RunSink).  Returns the terminate plane (reference
+// March one ray into the sink `out` (GenericOut, RunSink or SampleSink).  Returns the terminate plane (reference
 // grid.cu:274-275).
 template <class Boxes, class Out>
 NFA_HD float generic_march_ray(const Boxes& boxes, const OccView& occ, const float o[3], const float d[3],

@@ -210,6 +210,46 @@ class OccGridEstimator(AbstractEstimator):
                                                  early_stop_eps=early_stop_eps, alpha_thre=alpha_thre)
         return ray_indices[masks], t_starts[masks], t_ends[masks]
 
+    @torch.no_grad()
+    def render_test(
+        self,
+        rays_o: Tensor,  # [n_rays, 3]
+        rays_d: Tensor,  # [n_rays, 3]
+        rgb_sigma_fn: Callable,
+        max_samples: int,
+        near_plane: float = 0.0,
+        far_plane: float = 1e10,
+        render_step_size: float = 1e-3,
+        render_bkgd: Optional[Tensor] = None,
+        cone_angle: float = 0.0,
+        alpha_thre: float = 0.0,
+        early_stop_eps: float = 1e-4,
+    ) -> Tuple[Tensor, Tensor, Tensor, int]:
+        """Render an evaluation image with early ray termination: march every live ray a few samples at a time,
+        shade only those samples, composite them onto the running result and retire a ray once it is opaque
+        (opacity > 1 - early_stop_eps) or has left the grid, until no ray is live or `max_samples` samples per ray
+        have been asked for.  Field work stops where the surfaces are, and a round needs memory for at most
+        n_alive x n_samples samples.  Not part of nerfacc's API.
+
+        Its results are those of the test-mode loop of nerfacc's examples (examples/utils.py:267-439,
+        `render_image_with_occgrid_test`): the same rounds, the same samples handed to the field in each round,
+        and colours, opacities and depths of the same arithmetic, summed without atomics (so two runs give the same
+        image).  `rgb_sigma_fn(t_starts, t_ends, ray_indices) -> (rgbs (N, 3), sigmas (N,))` is `rendering`'s closure,
+        with ray indices into `rays_o`; it must return float32.  Returns (colors (R, 3), opacities (R, 1), depths (R, 1),
+        total_samples): depths are normalised by the opacity, `render_bkgd` is blended in where given, and
+        total_samples counts the samples that passed `alpha_thre`.
+
+        Each round waits for the GPU once, for its sample count (plus one wait at the end when `max_samples` stops
+        the loop, for the sample total).  `render_step_size <= 0` (one sample per cell) runs the loop over the public
+        functions instead.  Inference only."""
+        _lib.require_cuda(rays_o, "render_test")
+        if render_step_size > 0.0:
+            return _render_test_native(self, rays_o, rays_d, rgb_sigma_fn, int(max_samples), float(near_plane),
+                                       float(far_plane), float(render_step_size), render_bkgd, float(cone_angle),
+                                       float(alpha_thre), float(early_stop_eps))
+        return _render_test_public(self, rays_o, rays_d, rgb_sigma_fn, int(max_samples), near_plane, far_plane,
+                                   render_step_size, render_bkgd, cone_angle, alpha_thre, early_stop_eps)
+
     def _occs_mean(self) -> float:
         """`occs.mean()` (reference occ_grid.py:183), cached per version of the buffer: the reference pays a
         2M-element reduction and a host sync for it on every sampling call."""
@@ -403,6 +443,156 @@ def _visibility_compact(t_starts: Tensor, t_ends: Tensor, dens: Tensor, packed_i
     out_ri, out_ts, out_te = out_ri[:kept], out_ts[:kept], out_te[:kept]
     _stash_packed_info(out_ri, new_pi, n_rays)
     return out_ri, out_ts, out_te
+
+
+class _RenderTestScratch:
+    """Workspace, pinned status slot and event of render_test for one (device, stream); it only grows."""
+
+    def __init__(self, device):
+        self.device = device
+        self.workspace = None
+        self.status = torch.zeros(4, dtype=torch.int64).pin_memory()
+        self.status_np = self.status.numpy()  # same pinned memory
+        self.event = torch.cuda.Event()
+
+    def reserve(self, n_rays: int, min_samples: int) -> None:
+        need = _lib.load().nfa_render_test_workspace_bytes(n_rays, min_samples)
+        if self.workspace is None or self.workspace.numel() < need:
+            # zeroed: the kernels expect (and leave behind) zero arrival counters
+            self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
+
+
+_rt_scratch: dict = {}
+
+
+def _render_test_scratch(device, n_rays: int, min_samples: int) -> _RenderTestScratch:
+    key = (device, _lib.stream_ptr(device))  # per stream: stream order is what protects the workspace
+    sc = _rt_scratch.get(key)
+    if sc is None:
+        if len(_rt_scratch) >= 16:
+            _rt_scratch.clear()
+        sc = _rt_scratch[key] = _RenderTestScratch(device)
+    sc.reserve(n_rays, min_samples)
+    return sc
+
+
+def _render_test_native(est, rays_o, rays_d, rgb_sigma_fn, max_samples: int, near_plane: float, far_plane: float,
+                        step_size: float, render_bkgd, cone_angle: float, alpha_thre: float, early_stop_eps: float):
+    """OccGridEstimator.render_test on csrc/render_test.cu: per round march (one host wait, for the round's
+    n_alive / n_samples / sample count, all computed on the device), expand, the field, composite."""
+    from ..grid import _packed_grid, _sorted_crossings
+    from ..volrend import _f32c
+    device = rays_o.device
+    rays_o, rays_d = rays_o.contiguous().float(), rays_d.contiguous().float()
+    aabbs = est.aabbs.contiguous().float()
+    R = rays_o.shape[0]
+    colors = torch.zeros((R, 3), dtype=torch.float32, device=device)
+    opacities = torch.zeros((R, 1), dtype=torch.float32, device=device)
+    depths = torch.zeros((R, 1), dtype=torch.float32, device=device)
+    if R == 0:
+        return colors, opacities, depths, 0
+    bkgd = None if render_bkgd is None else render_bkgd.to(device=device, dtype=torch.float32).reshape(3).contiguous()
+    G, rx, ry, rz = (int(s) for s in est.binaries.shape)
+    occ = _packed_grid(est.binaries)
+    t_sorted, t_indices, hits = _sorted_crossings(rays_o, rays_d, aabbs, G)
+    min_samples = 1 if cone_angle == 0 else 4  # examples/utils.py:322
+    # `opacity <= 1 - early_stop_eps` compares in float32 (examples/utils.py:425): round the threshold once, here
+    opacity_thre = float(torch.tensor(1.0 - early_stop_eps, dtype=torch.float32))
+    sc = _render_test_scratch(device, R, min_samples)
+    ws, status = _lib.ptr(sc.workspace), sc.status_np
+    stream = torch.cuda.current_stream(device)
+    _lib.call("nfa_render_test_begin", device, R, min_samples, near_plane, ws)
+    iter_samples, k, total = 0, 0, None
+    while iter_samples < max_samples:
+        _lib.call("nfa_render_test_march", device, R, min_samples, k, _lib.ptr(rays_o), _lib.ptr(rays_d), far_plane, G,
+                  rx, ry, rz, _lib.ptr(occ.words), _lib.ptr(occ.coarse), _lib.ptr(aabbs), _lib.ptr(t_sorted),
+                  _lib.ptr(t_indices), _lib.ptr(hits), step_size, cone_angle, ws, _lib.ptr(sc.status))
+        sc.event.record(stream)
+        sc.event.synchronize()  # the round's one wait
+        n_alive, n_samples, n = int(status[0]), int(status[1]), int(status[2])
+        if n_alive == 0:
+            total = int(status[3])  # every composite has run: the kept total is complete
+            break
+        iter_samples += n_samples
+        ray_indices = torch.empty(n, dtype=torch.int64, device=device)
+        t_starts = torch.empty(n, dtype=torch.float32, device=device)
+        t_ends = torch.empty(n, dtype=torch.float32, device=device)
+        if n:
+            _lib.call("nfa_render_test_expand", device, R, min_samples, k, n_alive, n_samples, ws,
+                      _lib.ptr(ray_indices), _lib.ptr(t_starts), _lib.ptr(t_ends))
+        rgbs, sigmas = rgb_sigma_fn(t_starts, t_ends, ray_indices)
+        assert rgbs.shape == (n, 3), "rgbs must have shape (N, 3), got {}".format(tuple(rgbs.shape))
+        assert sigmas.shape == (n,), "sigmas must have shape (N,), got {}".format(tuple(sigmas.shape))
+        rgbs, sigmas = _f32c(rgbs.detach()), _f32c(sigmas.detach())
+        _lib.call("nfa_render_test_composite", device, R, min_samples, k, n_alive, n_samples, n, ws,
+                  _lib.ptr(t_starts), _lib.ptr(t_ends), _lib.ptr(rgbs), _lib.ptr(sigmas), alpha_thre, opacity_thre,
+                  _lib.ptr(colors), _lib.ptr(opacities), _lib.ptr(depths))
+        k += 1
+    _lib.call("nfa_render_test_finish", device, R, min_samples, ws, _lib.ptr(bkgd), _lib.ptr(colors),
+              _lib.ptr(opacities), _lib.ptr(depths), None if (total is not None or k == 0) else _lib.ptr(sc.status))
+    if total is None:
+        if k > 0:  # the sample budget ended the loop: the last composite's kept samples are still on the device
+            sc.event.record(stream)
+            sc.event.synchronize()
+            total = int(status[3])
+        else:
+            total = 0
+    return colors, opacities, depths, total
+
+
+def _render_test_public(est, rays_o, rays_d, rgb_sigma_fn, max_samples: int, near_plane, far_plane, step_size,
+                        render_bkgd, cone_angle, alpha_thre, early_stop_eps):
+    """render_test as the reference's loop over the public functions (examples/utils.py:314-439)."""
+    from ..grid import ray_aabb_intersect
+    from ..volrend import accumulate_along_rays_, render_weight_from_density
+    device, R = rays_o.device, rays_o.shape[0]
+    opacity = torch.zeros(R, 1, device=device)
+    depth = torch.zeros(R, 1, device=device)
+    rgb = torch.zeros(R, 3, device=device)
+    ray_mask = torch.ones(R, device=device).bool()
+    min_samples = 1 if cone_angle == 0 else 4
+    iter_samples = total_samples = 0
+    near_planes = torch.full_like(rays_o[..., 0], fill_value=near_plane)
+    far_planes = torch.full_like(rays_o[..., 0], fill_value=far_plane)
+    t_mins, t_maxs, hits = ray_aabb_intersect(rays_o, rays_d, est.aabbs)
+    n_grids = est.binaries.size(0)
+    if n_grids > 1:
+        t_sorted, t_indices = torch.sort(torch.cat([t_mins, t_maxs], -1), -1)
+    else:
+        t_sorted = torch.cat([t_mins, t_maxs], -1)
+        t_indices = torch.arange(0, n_grids * 2, device=device, dtype=torch.int64).expand(R, n_grids * 2)
+    opc_thre = 1 - early_stop_eps
+    while iter_samples < max_samples:
+        n_alive = int(ray_mask.sum().item())
+        if n_alive == 0:
+            break
+        n_samples = max(min(R // n_alive, 64), min_samples)
+        iter_samples += n_samples
+        intervals, samples, termination_planes = traverse_grids(
+            rays_o, rays_d, est.binaries, est.aabbs, near_planes, far_planes, step_size, cone_angle, n_samples, True,
+            ray_mask, t_sorted, t_indices, hits)
+        t_starts = intervals.vals[intervals.is_left]
+        t_ends = intervals.vals[intervals.is_right]
+        ray_indices = samples.ray_indices[samples.is_valid]
+        packed_info = samples.packed_info
+        rgbs, sigmas = rgb_sigma_fn(t_starts, t_ends, ray_indices)
+        weights, _, alphas = render_weight_from_density(t_starts, t_ends, sigmas, ray_indices=ray_indices, n_rays=R,
+                                                        prefix_trans=1 - opacity[ray_indices].squeeze(-1))
+        if alpha_thre > 0:
+            vis = alphas >= alpha_thre
+            ray_indices, rgbs, weights, t_starts, t_ends = (ray_indices[vis], rgbs[vis], weights[vis], t_starts[vis],
+                                                            t_ends[vis])
+        accumulate_along_rays_(weights, values=rgbs, ray_indices=ray_indices, outputs=rgb)
+        accumulate_along_rays_(weights, values=None, ray_indices=ray_indices, outputs=opacity)
+        accumulate_along_rays_(weights, values=(t_starts + t_ends)[..., None] / 2.0, ray_indices=ray_indices,
+                               outputs=depth)
+        near_planes = termination_planes
+        ray_mask = torch.logical_and(opacity.view(-1) <= opc_thre, packed_info[:, 1] == n_samples)
+        total_samples += ray_indices.shape[0]
+    if render_bkgd is not None:
+        rgb = rgb + render_bkgd * (1.0 - opacity)
+    depth = depth / opacity.clamp_min(torch.finfo(torch.float32).eps)
+    return rgb, opacity, depth, total_samples
 
 
 def _meshgrid3d(res: Tensor, device: Union[torch.device, str] = "cpu") -> Tensor:

@@ -324,6 +324,33 @@ int32_t nfa_visibility_compact(int32_t n_rays, int64_t n_samples, const int64_t*
                                int64_t* new_packed_info, int64_t* out_ray_indices, float* out_t_starts,
                                float* out_t_ends, int64_t* total_dev, int64_t* total_host, nfa_stream_t stream);
 
+/* The same filter in rounds (OccGridEstimator.sampling_until_opaque): the field runs on each live ray's next k
+ *   samples only (k a multiple of 32), and a ray stops being live once its next sample's transmittance fails
+ *   T >= early_stop_eps.  Every T, alpha and keep bit is nfa_visibility_compact's when densities are >= 0 (alphas in
+ *   [0, 1]).  The workspace (nfa_vis_rounds_workspace_bytes; 16-byte aligned, no state carried between calls) holds the live-ray lists, the per-ray carries and counts and the mask; it is owned by one stream.
+ *   status_host (pinned, [4]) = {n_alive, k, samples of the round, kept samples so far}, written for the next round
+ *   by begin and every step; n_alive == 0 ends the loop.  n_alive / round / n_with_samples come from it.
+ *   begin   every ray with samples live (in ray order, round 0, k = 32), mask zeroed.  n_with_samples = its n_alive.
+ *   gather  the round's closure inputs, in ray order: each live ray's next min(k, left) samples.
+ *   step    the closure's float32 outputs for those samples: mask bytes, kept counts and carries; the next round's
+ *           live list, k = 32 clamp(n_with_samples / n_alive, 1, 8) and sample count.
+ *   finish  the kept (ray_indices, t_starts, t_ends) compacted in ray order and their packed_info. */
+int64_t nfa_vis_rounds_workspace_bytes(int32_t n_rays, int64_t n_samples);
+int32_t nfa_vis_rounds_begin(int32_t n_rays, int64_t n_samples, const int64_t* packed_info, int32_t from_alpha,
+                             void* workspace, int64_t* status_host, nfa_stream_t stream);
+int32_t nfa_vis_rounds_gather(int32_t n_rays, int64_t n_samples, int32_t round, int32_t n_alive,
+                              const int64_t* packed_info, const float* t_starts, const float* t_ends,
+                              const void* workspace, int64_t* out_ray_indices, float* out_t_starts, float* out_t_ends,
+                              nfa_stream_t stream);
+int32_t nfa_vis_rounds_step(int32_t n_rays, int64_t n_samples, int32_t round, int32_t n_alive,
+                            int32_t n_with_samples, const int64_t* packed_info, const float* t_starts,
+                            const float* t_ends, const float* sigmas_or_alphas, int32_t from_alpha,
+                            float early_stop_eps, float alpha_thre, void* workspace, int64_t* status_host,
+                            nfa_stream_t stream);
+int32_t nfa_vis_rounds_finish(int32_t n_rays, int64_t n_samples, const int64_t* packed_info, const float* t_starts,
+                              const float* t_ends, const void* workspace, int64_t* new_packed_info,
+                              int64_t* out_ray_indices, float* out_t_starts, float* out_t_ends, nfa_stream_t stream);
+
 /* ----------------------------------------------------------------------- */
 /* Early-terminated test-time rendering (OccGridEstimator.render_test)      */
 /* ----------------------------------------------------------------------- */

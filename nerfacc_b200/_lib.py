@@ -57,7 +57,13 @@ SIGNATURES = {
     "nfa_visibility_workspace_bytes": (_c_i64, [_c_i32, _c_i64]),
     "nfa_visibility_compact": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_i32, _c_f32, _c_f32]
                                + [_c_ptr] * 8),
-    "nfa_render_test_workspace_bytes": (_c_i64, [_c_i32, _c_i32]),
+    "nfa_vis_rounds_workspace_bytes": (_c_i64, [_c_i32, _c_i64]),
+    "nfa_vis_rounds_begin": (_c_i32, [_c_i32, _c_i64, _c_ptr, _c_i32, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_vis_rounds_gather": (_c_i32, [_c_i32, _c_i64, _c_i32, _c_i32] + [_c_ptr] * 8),
+    "nfa_vis_rounds_step": (_c_i32, [_c_i32, _c_i64, _c_i32, _c_i32, _c_i32, _c_ptr, _c_ptr, _c_ptr, _c_ptr, _c_i32,
+                                     _c_f32, _c_f32, _c_ptr, _c_ptr, _c_ptr]),
+    "nfa_vis_rounds_finish": (_c_i32, [_c_i32, _c_i64] + [_c_ptr] * 9),
+    "nfa_render_test_workspace_bytes":(_c_i64, [_c_i32, _c_i32]),
     "nfa_render_test_begin": (_c_i32, [_c_i32, _c_i32, _c_f32, _c_ptr, _c_ptr]),
     "nfa_render_test_march": (_c_i32, [_c_i32, _c_i32, _c_i32, _c_ptr, _c_ptr, _c_f32, _c_i32, _c_i32, _c_i32, _c_i32]
                               + [_c_ptr] * 6 + [_c_f32, _c_f32, _c_ptr, _c_ptr, _c_ptr]),

@@ -17,6 +17,7 @@
 
 #include "../../include/nerfacc_b200.h"
 #include "sm_count.cuh"
+#include "vis_block.cuh"
 
 namespace nfa {
 
@@ -376,32 +377,6 @@ __global__ void __launch_bounds__(kPackTile) pack_scan_kernel(int32_t n_rays,
 // synchronising boolean mask-selects; here: mask + per-ray counts, the two-level scan of
 // pack_info, and a ballot compaction that writes the kept samples and their packed_info.
 // ---------------------------------------------------------------------------
-// exp as the reference evaluates it: ATen's exp kernel calls the CUDA math library's expf (not the ex2.approx
-// shortcut): the keep / drop decision compares T and alpha with thresholds, so the last bit matters.
-__device__ __forceinline__ float vis_exp_neg(float x) { return expf(-x); }
-
-// Inclusive scan of one 32-element block in the summation ORDER of the reference's packed scan kernel
-// (include/utils_scan.cuh:146-263, launched 16 x 32 => blocks of 2 x 16 = 32 elements): the running total of the
-// previous blocks is folded into element 0, then a Brent-Kung up-sweep / down-sweep.  Float addition is not
-// associative, and `sampling(sigma_fn=...)` thresholds the result, so the tree is reproduced step by step
-// (9 shuffles instead of the 5 of a Kogge-Stone scan; the filter is memory-bound).
-template <bool kProd>
-__device__ __forceinline__ float ref_block_scan(float x, float carry, int lane)
-{
-    if (lane == 0) x = kProd ? x * carry : x + carry;  // utils_scan.cuh:196-198
-#pragma unroll
-    for (int d = 1; d <= 16; d <<= 1) {  // up-sweep, :203-209
-        const float y = __shfl_up_sync(kFullMask, x, d);
-        if (((lane + 1) & (2 * d - 1)) == 0) x = kProd ? y * x : y + x;
-    }
-#pragma unroll
-    for (int d = 8; d >= 1; d >>= 1) {  // down-sweep, :212-218
-        const float y = __shfl_up_sync(kFullMask, x, d);
-        if (((lane + 1) & (2 * d - 1)) == d && lane + 1 > d) x = kProd ? y * x : y + x;
-    }
-    return x;
-}
-
 template <bool kAlpha>
 __global__ void __launch_bounds__(kScanWarps * 32) vis_mask_kernel(int32_t n_rays,
                                                                    const int64_t* __restrict__ packed_info,
@@ -416,34 +391,8 @@ __global__ void __launch_bounds__(kScanWarps * 32) vis_mask_kernel(int32_t n_ray
         const longlong2 pi = *reinterpret_cast<const longlong2*>(packed_info + 2 * (int64_t)r);
         const int64_t start = pi.x, n = pi.y;
         float carry = kAlpha ? 1.0f : 0.0f;  // `init` of the reference kernel; then the previous blocks' total
-        unsigned kept = 0;
-        for (int64_t base = 0; base < n; base += 32) {
-            const int64_t i = start + base + lane;
-            const bool valid = base + lane < n;
-            float T, a;
-            if (!kAlpha) {
-                // volrend.py:271-275: sigmas_dt = sigmas * (t_ends - t_starts); alphas = 1 - exp(-sigmas_dt);
-                // trans = exp(-exclusive_sum(sigmas_dt))
-                const float sd = valid ? __fmul_rn(__ldg(dens + i), __fsub_rn(__ldg(t_ends + i), __ldg(t_starts + i))) : 0.f;
-                const float incl = ref_block_scan<false>(sd, carry, lane);
-                float excl = __shfl_up_sync(kFullMask, incl, 1);
-                if (lane == 0) excl = carry;
-                T = vis_exp_neg(excl);
-                a = __fsub_rn(1.0f, vis_exp_neg(sd));
-                carry = __shfl_sync(kFullMask, incl, 31);
-            } else {
-                // volrend.py:208-210: trans = exclusive_prod(1 - alphas)
-                a = valid ? __ldg(dens + i) : 0.f;
-                const float incl = ref_block_scan<true>(valid ? __fsub_rn(1.0f, a) : 1.0f, carry, lane);
-                float excl = __shfl_up_sync(kFullMask, incl, 1);
-                if (lane == 0) excl = carry;
-                T = excl;
-                carry = __shfl_sync(kFullMask, incl, 31);
-            }
-            const bool keep = valid && (T >= early_stop_eps) && (!(alpha_thre > 0.0f) || a >= alpha_thre);
-            if (valid) mask[i] = keep ? 1 : 0;
-            kept += __popc(__ballot_sync(kFullMask, keep));
-        }
+        const unsigned kept =
+            vis_blocks<kAlpha>(t_starts, t_ends, dens, start, n, lane, carry, early_stop_eps, alpha_thre, mask, 0);
         if (lane == 0) counts[r] = kept;
     }
 }
@@ -475,6 +424,197 @@ __global__ void __launch_bounds__(kScanWarps * 32) vis_compact_kernel(int32_t n_
             }
             dst += __popc(b);
         }
+    }
+}
+
+// ---------------------------------------------------------------------------
+// Visibility filter in rounds (OccGridEstimator.sampling_until_opaque): the field closure runs on each live ray's
+// next k samples only, and a ray stops being live once the transmittance its next sample would get fails
+// T >= early_stop_eps.  Each round advances a ray by whole 32-sample blocks from its first sample (k is a multiple
+// of 32) and carries the block total across rounds, so every T, alpha and keep bit is the one-shot filter's
+// (vis_blocks, vis_block.cuh).  Per round: a gather of the closure's inputs, the closure, the step (mask bytes,
+// kept counts, carry, live flag), the exclusive scan of the live flags (pack_tilesum / pack_scan), a scatter of the
+// next live list with each slot's sample count, and the scan of those counts, whose total goes to a pinned status
+// slot with the next round's n_alive, k and the running kept total.  The finish is vis_compact_kernel over the
+// kept counts' scan; mask bytes of samples that were never evaluated stay 0 from the zeroing at the start.
+// See DESIGN.md section 4.12.
+// ---------------------------------------------------------------------------
+constexpr int kRoundBlock = 32;      // samples per scan block: a round evaluates whole blocks of every live ray
+constexpr int kRoundMaxBlocks = 8;   // k_r = 32 clamp(rays with samples / n_alive, 1, 8)
+
+// Workspace (offsets 16-byte aligned) for R rays and N samples:
+//   header (64 B): i64 live rays after the current step (scan total), u64 kept samples so far
+//   lists [2][R] i32     live rays of the even / odd rounds, ascending
+//   carry [R] f32        per ray: total of its evaluated blocks
+//   done [R] i64         per ray: samples evaluated
+//   counts [R] u64       per ray: samples kept (what pack_scan turns into the new packed_info)
+//   live [R] u64         per slot of the current round: stays live (0 / 1)
+//   live_pi [R][2] i64   exclusive scan of `live` (slot's rank among the live slots, flag)
+//   cnt [R] u64          per slot of the next round: its sample count
+//   plan [R][2] i64      exclusive scan of `cnt`: (offset into the closure's inputs, count)
+//   tile_sums [T] u64    T = ceil(R / kPackTile)
+//   mask [N] u8          keep byte of every sample
+struct VisRoundsWs {
+    int64_t* n_next;
+    unsigned long long* kept;
+    int32_t* lists;
+    float* carry;
+    int64_t* done;
+    unsigned long long* counts;
+    unsigned long long* live;
+    int64_t* live_pi;
+    unsigned long long* cnt;
+    int64_t* plan;
+    unsigned long long* tile_sums;
+    uint8_t* mask;
+    int32_t n_rays;
+};
+
+static int64_t vis_rounds_bytes(int32_t R, int64_t N, VisRoundsWs* w, char* base)
+{
+    const int64_t T = (R + kPackTile - 1) / kPackTile;
+    int64_t at = 64;
+    auto take = [&](int64_t bytes) {
+        char* p = base ? base + at : nullptr;
+        at += (bytes + 15) & ~(int64_t)15;
+        return p;
+    };
+    char* lists = take(8 * (int64_t)R);
+    char* carry = take(4 * (int64_t)R);
+    char* done = take(8 * (int64_t)R);
+    char* counts = take(8 * (int64_t)R);
+    char* live = take(8 * (int64_t)R);
+    char* live_pi = take(16 * (int64_t)R);
+    char* cnt = take(8 * (int64_t)R);
+    char* plan = take(16 * (int64_t)R);
+    char* tile_sums = take(8 * T);
+    char* mask = take(N);
+    if (w) {
+        w->n_next = (int64_t*)base;
+        w->kept = (unsigned long long*)(base + 8);
+        w->lists = (int32_t*)lists;
+        w->carry = (float*)carry;
+        w->done = (int64_t*)done;
+        w->counts = (unsigned long long*)counts;
+        w->live = (unsigned long long*)live;
+        w->live_pi = (int64_t*)live_pi;
+        w->cnt = (unsigned long long*)cnt;
+        w->plan = (int64_t*)plan;
+        w->tile_sums = (unsigned long long*)tile_sums;
+        w->mask = (uint8_t*)mask;
+        w->n_rays = R;
+    }
+    return at;
+}
+
+static VisRoundsWs vis_rounds_view(void* base, int32_t R, int64_t N)
+{
+    VisRoundsWs w;
+    vis_rounds_bytes(R, N, &w, (char*)base);
+    return w;
+}
+
+// Every ray: nothing evaluated or kept, the initial carry; slot r of the "round before round 0" is ray r, live when
+// it has samples.
+__global__ void __launch_bounds__(256) vis_rounds_init_kernel(VisRoundsWs ws, const int64_t* __restrict__ packed_info,
+                                                              float carry0)
+{
+    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < ws.n_rays; r += gridDim.x * blockDim.x) {
+        ws.carry[r] = carry0;
+        ws.done[r] = 0;
+        ws.counts[r] = 0ull;
+        ws.live[r] = packed_info[2 * (int64_t)r + 1] > 0 ? 1ull : 0ull;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *ws.kept = 0ull;
+}
+
+// Warp per live slot: the slot's next plan[i].y samples (from the ray's first unevaluated one) -> the closure's
+// inputs at offset plan[i].x.
+__global__ void __launch_bounds__(kScanWarps * 32) vis_rounds_gather_kernel(VisRoundsWs ws, int32_t round,
+                                                                            int32_t n_alive,
+                                                                            const int64_t* __restrict__ packed_info,
+                                                                            const float* __restrict__ t_starts,
+                                                                            const float* __restrict__ t_ends,
+                                                                            int64_t* __restrict__ out_ray,
+                                                                            float* __restrict__ out_ts,
+                                                                            float* __restrict__ out_te)
+{
+    const int lane = threadIdx.x & 31;
+    const int32_t* list = ws.lists + (int64_t)(round & 1) * ws.n_rays;
+    for (int i = blockIdx.x * kScanWarps + (threadIdx.x >> 5); i < n_alive; i += gridDim.x * kScanWarps) {
+        const int r = list[i];
+        const longlong2 pl = *reinterpret_cast<const longlong2*>(ws.plan + 2 * (int64_t)i);
+        const int64_t src = packed_info[2 * (int64_t)r] + ws.done[r];
+        for (int64_t j = lane; j < pl.y; j += 32) {
+            out_ray[pl.x + j] = r;
+            out_ts[pl.x + j] = __ldg(t_starts + src + j);
+            out_te[pl.x + j] = __ldg(t_ends + src + j);
+        }
+    }
+}
+
+// Warp per live slot: the filter over the slot's samples of this round (the closure's inputs and outputs at offset
+// plan[i].x), their mask bytes at the ray's sample positions, the kept count, the carry, and whether the ray stays
+// live: samples left, and its next sample's T passes.
+template <bool kAlpha>
+__global__ void __launch_bounds__(kScanWarps * 32) vis_rounds_step_kernel(VisRoundsWs ws, int32_t round,
+                                                                          int32_t n_alive,
+                                                                          const int64_t* __restrict__ packed_info,
+                                                                          const float* __restrict__ t_starts,
+                                                                          const float* __restrict__ t_ends,
+                                                                          const float* __restrict__ dens,
+                                                                          float early_stop_eps, float alpha_thre)
+{
+    const int lane = threadIdx.x & 31;
+    const int32_t* list = ws.lists + (int64_t)(round & 1) * ws.n_rays;
+    unsigned long long kept_warp = 0;
+    for (int i = blockIdx.x * kScanWarps + (threadIdx.x >> 5); i < n_alive; i += gridDim.x * kScanWarps) {
+        const int r = list[i];
+        const longlong2 pl = *reinterpret_cast<const longlong2*>(ws.plan + 2 * (int64_t)i);
+        const longlong2 pi = *reinterpret_cast<const longlong2*>(packed_info + 2 * (int64_t)r);
+        const int64_t d0 = ws.done[r];
+        float carry = ws.carry[r];
+        const unsigned kept = vis_blocks<kAlpha>(t_starts, t_ends, dens, pl.x, pl.y, lane, carry, early_stop_eps,
+                                                 alpha_thre, ws.mask, pi.x + d0 - pl.x);
+        kept_warp += kept;
+        if (lane == 0) {
+            const int64_t d1 = d0 + pl.y;
+            ws.counts[r] += kept;
+            ws.done[r] = d1;
+            ws.carry[r] = carry;
+            ws.live[i] = (d1 < pi.y && vis_next_passes<kAlpha>(carry, early_stop_eps)) ? 1ull : 0ull;
+        }
+    }
+    if (lane == 0 && kept_warp) atomicAdd(ws.kept, kept_warp);
+}
+
+// Thread per slot of the round just stepped (`first`: the rays themselves, before round 0): a live slot moves to its
+// rank in the next round's list and gets min(k, samples left) samples; the others zero the tail of `cnt`, so that
+// the scan over all n_cur entries totals the next round's samples.  Slot 0 also publishes the next round's
+// {n_alive, k, -, kept samples so far}; the scan of `cnt` fills in the sample count.
+__global__ void __launch_bounds__(256) vis_rounds_scatter_kernel(VisRoundsWs ws, int32_t round, int32_t n_cur,
+                                                                 int32_t first, int32_t n_with_samples,
+                                                                 const int64_t* __restrict__ packed_info,
+                                                                 int64_t* status_host)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_cur) return;
+    const int64_t n_next = *ws.n_next;
+    const int64_t q = n_next > 0 ? n_with_samples / n_next : 1;
+    const int64_t k = first ? kRoundBlock : kRoundBlock * (q < 1 ? 1 : (q > kRoundMaxBlocks ? kRoundMaxBlocks : q));
+    const longlong2 lb = *reinterpret_cast<const longlong2*>(ws.live_pi + 2 * (int64_t)i);
+    if (lb.y) {
+        const int r = first ? i : ws.lists[(int64_t)(round & 1) * ws.n_rays + i];
+        ws.lists[(int64_t)(first ? 0 : (round + 1) & 1) * ws.n_rays + lb.x] = r;
+        const int64_t left = packed_info[2 * (int64_t)r + 1] - ws.done[r];
+        ws.cnt[lb.x] = (unsigned long long)(left < k ? left : k);
+    } else {
+        ws.cnt[n_next + i - lb.x] = 0ull;
+    }
+    if (i == 0) {  // read by the host after it has waited for the scan behind this kernel
+        status_host[0] = n_next;
+        status_host[1] = n_next > 0 ? k : 0;
+        status_host[3] = (int64_t)*ws.kept;
     }
 }
 
@@ -641,6 +781,119 @@ int32_t nfa_visibility_compact(int32_t n_rays, int64_t n_samples, const int64_t*
     if (n_samples > 0)
         vis_compact_kernel<<<blocks, kScanWarps * 32, 0, s>>>(n_rays, packed_info, new_packed_info, mask, t_starts, t_ends,
                                                               out_ray_indices, out_t_starts, out_t_ends);
+    return launch_status_s();
+}
+
+
+int64_t nfa_vis_rounds_workspace_bytes(int32_t n_rays, int64_t n_samples)
+{
+    if (n_rays < 1 || n_samples < 0) return 0;
+    return vis_rounds_bytes(n_rays, n_samples, nullptr, nullptr);
+}
+
+static void vis_rounds_plan(const VisRoundsWs& w, int32_t round, int32_t n_cur, int32_t first, int32_t n_with_samples,
+                            const int64_t* packed_info, int64_t* status_host, cudaStream_t s)
+{
+    const int tiles = (n_cur + kPackTile - 1) / kPackTile;
+    pack_tilesum_kernel<<<tiles, kPackTile, 0, s>>>(n_cur, w.live, w.tile_sums);
+    pack_scan_kernel<<<tiles, kPackTile, 0, s>>>(n_cur, w.live, w.tile_sums, w.live_pi, w.n_next, nullptr);
+    vis_rounds_scatter_kernel<<<(n_cur + 255) / 256, 256, 0, s>>>(w, round, n_cur, first, n_with_samples, packed_info,
+                                                                  status_host);
+    pack_tilesum_kernel<<<tiles, kPackTile, 0, s>>>(n_cur, w.cnt, w.tile_sums);
+    pack_scan_kernel<<<tiles, kPackTile, 0, s>>>(n_cur, w.cnt, w.tile_sums, w.plan, nullptr, status_host + 2);
+}
+
+static inline bool aligned16(const void* p) { return (((uintptr_t)p) & 15u) == 0; }
+
+int32_t nfa_vis_rounds_begin(int32_t n_rays, int64_t n_samples, const int64_t* packed_info, int32_t from_alpha,
+                             void* workspace, int64_t* status_host, nfa_stream_t stream)
+{
+    if (n_rays < 1 || n_samples < 0) return NFA_ERR_ARG;
+    if (!packed_info || !workspace || !status_host || !aligned16(packed_info) || !aligned16(workspace))
+        return NFA_ERR_ARG;
+    cudaStream_t s = (cudaStream_t)stream;
+    const VisRoundsWs w = vis_rounds_view(workspace, n_rays, n_samples);
+    if (n_samples > 0) {
+        const cudaError_t e = cudaMemsetAsync(w.mask, 0, (size_t)n_samples, s);
+        if (e != cudaSuccess) return (int32_t)e;
+    }
+    const int need = (n_rays + 255) / 256;
+    vis_rounds_init_kernel<<<need < kNumSMs * 8 ? need : kNumSMs * 8, 256, 0, s>>>(w, packed_info,
+                                                                                  from_alpha ? 1.0f : 0.0f);
+    vis_rounds_plan(w, 0, n_rays, 1, 0, packed_info, status_host, s);
+    return launch_status_s();
+}
+
+static bool vis_rounds_round_ok(int32_t n_rays, int64_t n_samples, int32_t round, int32_t n_alive)
+{
+    return n_rays >= 1 && n_samples >= 0 && round >= 0 && n_alive >= 1 && n_alive <= n_rays;
+}
+
+int32_t nfa_vis_rounds_gather(int32_t n_rays, int64_t n_samples, int32_t round, int32_t n_alive,
+                              const int64_t* packed_info, const float* t_starts, const float* t_ends,
+                              const void* workspace, int64_t* out_ray_indices, float* out_t_starts, float* out_t_ends,
+                              nfa_stream_t stream)
+{
+    if (!vis_rounds_round_ok(n_rays, n_samples, round, n_alive)) return NFA_ERR_ARG;
+    if (!packed_info || !t_starts || !t_ends || !workspace || !out_ray_indices || !out_t_starts || !out_t_ends ||
+        !aligned16(workspace))
+        return NFA_ERR_ARG;
+    const int need = (n_alive + kScanWarps - 1) / kScanWarps;
+    vis_rounds_gather_kernel<<<need < kNumSMs * 8 ? need : kNumSMs * 8, kScanWarps * 32, 0, (cudaStream_t)stream>>>(
+        vis_rounds_view(const_cast<void*>(workspace), n_rays, n_samples), round, n_alive, packed_info, t_starts,
+        t_ends, out_ray_indices, out_t_starts, out_t_ends);
+    return launch_status_s();
+}
+
+int32_t nfa_vis_rounds_step(int32_t n_rays, int64_t n_samples, int32_t round, int32_t n_alive,
+                            int32_t n_with_samples, const int64_t* packed_info, const float* t_starts,
+                            const float* t_ends, const float* sigmas_or_alphas, int32_t from_alpha,
+                            float early_stop_eps, float alpha_thre, void* workspace, int64_t* status_host,
+                            nfa_stream_t stream)
+{
+    if (!vis_rounds_round_ok(n_rays, n_samples, round, n_alive) || n_with_samples < n_alive ||
+        n_with_samples > n_rays)
+        return NFA_ERR_ARG;
+    if (!packed_info || !t_starts || !t_ends || !sigmas_or_alphas || !workspace || !status_host ||
+        !aligned16(workspace))
+        return NFA_ERR_ARG;
+    cudaStream_t s = (cudaStream_t)stream;
+    const VisRoundsWs w = vis_rounds_view(workspace, n_rays, n_samples);
+    const int need = (n_alive + kScanWarps - 1) / kScanWarps;
+    const int blocks = need < kNumSMs * 8 ? need : kNumSMs * 8;
+    if (from_alpha)
+        vis_rounds_step_kernel<true><<<blocks, kScanWarps * 32, 0, s>>>(w, round, n_alive, packed_info, t_starts,
+                                                                        t_ends, sigmas_or_alphas, early_stop_eps,
+                                                                        alpha_thre);
+    else
+        vis_rounds_step_kernel<false><<<blocks, kScanWarps * 32, 0, s>>>(w, round, n_alive, packed_info, t_starts,
+                                                                         t_ends, sigmas_or_alphas, early_stop_eps,
+                                                                         alpha_thre);
+    vis_rounds_plan(w, round, n_alive, 0, n_with_samples, packed_info, status_host, s);
+    return launch_status_s();
+}
+
+int32_t nfa_vis_rounds_finish(int32_t n_rays, int64_t n_samples, const int64_t* packed_info, const float* t_starts,
+                              const float* t_ends, const void* workspace, int64_t* new_packed_info,
+                              int64_t* out_ray_indices, float* out_t_starts, float* out_t_ends, nfa_stream_t stream)
+{
+    if (n_rays < 1 || n_samples < 0) return NFA_ERR_ARG;
+    if (!packed_info || !workspace || !new_packed_info || !aligned16(workspace) || !aligned16(packed_info) ||
+        !aligned16(new_packed_info))
+        return NFA_ERR_ARG;
+    if (n_samples > 0 && (!t_starts || !t_ends || !out_ray_indices || !out_t_starts || !out_t_ends))
+        return NFA_ERR_ARG;
+    cudaStream_t s = (cudaStream_t)stream;
+    const VisRoundsWs w = vis_rounds_view(const_cast<void*>(workspace), n_rays, n_samples);
+    const int tiles = (n_rays + kPackTile - 1) / kPackTile;
+    pack_tilesum_kernel<<<tiles, kPackTile, 0, s>>>(n_rays, w.counts, w.tile_sums);
+    pack_scan_kernel<<<tiles, kPackTile, 0, s>>>(n_rays, w.counts, w.tile_sums, new_packed_info, nullptr, nullptr);
+    if (n_samples > 0) {
+        const int need = (n_rays + kScanWarps - 1) / kScanWarps;
+        vis_compact_kernel<<<need < kNumSMs * 8 ? need : kNumSMs * 8, kScanWarps * 32, 0, s>>>(
+            n_rays, packed_info, new_packed_info, w.mask, t_starts, t_ends, out_ray_indices, out_t_starts,
+            out_t_ends);
+    }
     return launch_status_s();
 }
 

@@ -163,11 +163,72 @@ class OccGridEstimator(AbstractEstimator):
     ) -> Tuple[Tensor, Tensor, Tensor]:
         """Second half of :meth:`sampling`: wait for the traversal's sample count, return the samples (after the
         optional visibility filter)."""
+        res = self._finish_march(ticket)
+        return self._drop_invisible(res.ray_indices, res.t_starts, res.t_ends, res.packed_info, sigma_fn, alpha_fn,
+                                    early_stop_eps, alpha_thre)
+
+    def _finish_march(self, ticket):
         res = ticket.finish()
         # ~6% head-room over the last batch; re-measured every call
         self._capacity_hint = res.n_samples + (res.n_samples >> 4) + 1024
-        return self._drop_invisible(res.ray_indices, res.t_starts, res.t_ends, res.packed_info, sigma_fn, alpha_fn,
-                                    early_stop_eps, alpha_thre)
+        return res
+
+    @torch.no_grad()
+    def sampling_until_opaque(
+        self,
+        rays_o: Tensor,  # [n_rays, 3]
+        rays_d: Tensor,  # [n_rays, 3]
+        sigma_fn: Optional[Callable] = None,
+        alpha_fn: Optional[Callable] = None,
+        near_plane: float = 0.0,
+        far_plane: float = 1e10,
+        t_min: Optional[Tensor] = None,  # [n_rays]
+        t_max: Optional[Tensor] = None,  # [n_rays]
+        render_step_size: float = 1e-3,
+        early_stop_eps: float = 1e-4,
+        alpha_thre: float = 0.0,
+        stratified: bool = False,
+        cone_angle: float = 0.0,
+    ) -> Tuple[Tensor, Tensor, Tensor]:
+        """:meth:`sampling` with the visibility filter's field evaluated in rounds: each round hands the closure the
+        next k samples of every ray that is still live (k a multiple of 32, from 32 up to 256 as rays retire), and a
+        ray retires once the transmittance its next sample would get fails T >= early_stop_eps.  Behind an opaque
+        surface the field is no longer evaluated, where :meth:`sampling` evaluates it on every marched sample and
+        then drops those samples.  Same arguments, defaults and return value as :meth:`sampling`:
+        (ray_indices, t_starts, t_ends), grouped by ray, with their packed_info attached.  Not part of nerfacc's API.
+
+        The results are bit-identical to ``sampling(...)`` with the same arguments (and the same RNG state when
+        `stratified`) when
+          - the closure is batch-invariant: each sample's output does not depend on which other samples share the
+            call.  Elementwise torch ops are; a cuBLAS MLP may not be;
+          - densities are >= 0 and alphas lie in [0, 1], as every activation of nerfacc's examples gives.
+        The samples are those of :meth:`sampling`'s march.  Each round advances a ray by whole 32-sample blocks from
+        its first sample and carries the transmittance scan across rounds, so every T, alpha and keep bit is the
+        one-shot filter's; once T fails the threshold it fails for every later sample of the ray too.
+
+        The closure is called once per round, never with zero samples.  Its inputs are grouped by ray in ascending
+        order, each ray's samples in order, with indices into `rays_o`; each sample is handed over at most once.  It
+        must return float32 (anything else raises RuntimeError) of shape (N,).  The host waits for the GPU once for
+        the march, once per round and once after the last round.
+
+        Without a closure, with early_stop_eps <= 0 (no ray can retire) or render_step_size <= 0 this is
+        :meth:`sampling` itself (one closure call)."""
+        _lib.require_cuda(rays_o, "sampling_until_opaque")
+        kw = dict(near_plane=near_plane, far_plane=far_plane, t_min=t_min, t_max=t_max,
+                  render_step_size=render_step_size, stratified=stratified, cone_angle=cone_angle)
+        if (sigma_fn is None and alpha_fn is None) or not (early_stop_eps > 0.0) or not (render_step_size > 0.0) \
+                or not (cone_angle >= 0.0):
+            return self.sampling(rays_o, rays_d, sigma_fn=sigma_fn, alpha_fn=alpha_fn, early_stop_eps=early_stop_eps,
+                                 alpha_thre=alpha_thre, **kw)
+        res = self._finish_march(self.sampling_begin(rays_o, rays_d, **kw))
+        if res.t_starts.shape[0] == 0 or res.packed_info.shape[0] == 0:  # nothing to evaluate: sampling's own path
+            return self._drop_invisible(res.ray_indices, res.t_starts, res.t_ends, res.packed_info, sigma_fn,
+                                        alpha_fn, early_stop_eps, alpha_thre)
+        if alpha_thre > 0.0:
+            alpha_thre = min(alpha_thre, self._occs_mean())
+        use_sigma = sigma_fn is not None
+        return _visibility_rounds(res.t_starts, res.t_ends, res.packed_info, sigma_fn if use_sigma else alpha_fn,
+                                  not use_sigma, float(early_stop_eps), float(alpha_thre))
 
     @staticmethod
     def _ray_planes(rays_o, near_plane, far_plane, t_min, t_max, stratified, render_step_size, always: bool):
@@ -445,8 +506,60 @@ def _visibility_compact(t_starts: Tensor, t_ends: Tensor, dens: Tensor, packed_i
     return out_ri, out_ts, out_te
 
 
-class _RenderTestScratch:
-    """Workspace, pinned status slot and event of render_test for one (device, stream); it only grows."""
+def _visibility_rounds(t_starts: Tensor, t_ends: Tensor, packed_info: Tensor, fn: Callable, from_alpha: bool,
+                       early_stop_eps: float, alpha_thre: float):
+    """The visibility filter in rounds (csrc/scan.cu, nfa_vis_rounds_*): per round one host wait (for the round's
+    live rays and sample count, computed on the device), the gather of the closure's inputs, the closure, the step.
+    Returns the kept (ray_indices, t_starts, t_ends) with their packed_info attached."""
+    from ..volrend import _f32c
+    device = t_starts.device
+    n, n_rays = t_starts.shape[0], packed_info.shape[0]
+    pi = packed_info.contiguous()
+    if pi.dtype != torch.int64:
+        pi = pi.to(torch.int64)
+    ts, te = t_starts.contiguous(), t_ends.contiguous()
+    sc = _stream_scratch(_vr_scratch, device)
+    sc.reserve(_lib.load().nfa_vis_rounds_workspace_bytes(n_rays, n))
+    ws, status = _lib.ptr(sc.workspace), sc.status_np
+    stream = torch.cuda.current_stream(device)
+    _lib.call("nfa_vis_rounds_begin", device, n_rays, n, _lib.ptr(pi), int(from_alpha), ws, _lib.ptr(sc.status))
+    rnd, n_with_samples = 0, -1
+    while True:
+        sc.event.record(stream)
+        sc.event.synchronize()  # the round's one wait: its live rays, sample count and the kept total so far
+        n_alive, m = int(status[0]), int(status[2])
+        if rnd == 0:
+            n_with_samples = n_alive
+        if n_alive == 0:
+            kept = int(status[3])
+            break
+        ray_indices = torch.empty(m, dtype=torch.int64, device=device)
+        r_starts = torch.empty(m, dtype=torch.float32, device=device)
+        r_ends = torch.empty(m, dtype=torch.float32, device=device)
+        _lib.call("nfa_vis_rounds_gather", device, n_rays, n, rnd, n_alive, _lib.ptr(pi), _lib.ptr(ts), _lib.ptr(te),
+                  ws, _lib.ptr(ray_indices), _lib.ptr(r_starts), _lib.ptr(r_ends))
+        dens = fn(r_starts, r_ends, ray_indices)
+        assert dens.shape == r_starts.shape, "{} must have shape of (N,)! Got {}".format(
+            "alphas" if from_alpha else "sigmas", dens.shape)
+        dens = _f32c(dens.detach())
+        _lib.call("nfa_vis_rounds_step", device, n_rays, n, rnd, n_alive, n_with_samples, _lib.ptr(pi),
+                  _lib.ptr(r_starts), _lib.ptr(r_ends), _lib.ptr(dens), int(from_alpha), early_stop_eps, alpha_thre,
+                  ws, _lib.ptr(sc.status))
+        rnd += 1
+    new_pi = torch.empty((n_rays, 2), dtype=torch.int64, device=device)
+    out_ri = torch.empty(max(kept, 1), dtype=torch.int64, device=device)
+    out_ts = torch.empty(max(kept, 1), dtype=torch.float32, device=device)
+    out_te = torch.empty(max(kept, 1), dtype=torch.float32, device=device)
+    _lib.call("nfa_vis_rounds_finish", device, n_rays, n, _lib.ptr(pi), _lib.ptr(ts), _lib.ptr(te), ws,
+              _lib.ptr(new_pi), _lib.ptr(out_ri), _lib.ptr(out_ts), _lib.ptr(out_te))
+    out_ri, out_ts, out_te = out_ri[:kept], out_ts[:kept], out_te[:kept]
+    _stash_packed_info(out_ri, new_pi, n_rays)
+    return out_ri, out_ts, out_te
+
+
+class _StreamScratch:
+    """Workspace, pinned status slot and event of a loop in rounds (render_test, sampling_until_opaque) for one
+    (device, stream); the workspace only grows."""
 
     def __init__(self, device):
         self.device = device
@@ -455,24 +568,29 @@ class _RenderTestScratch:
         self.status_np = self.status.numpy()  # same pinned memory
         self.event = torch.cuda.Event()
 
-    def reserve(self, n_rays: int, min_samples: int) -> None:
-        need = _lib.load().nfa_render_test_workspace_bytes(n_rays, min_samples)
+    def reserve(self, need: int) -> None:
         if self.workspace is None or self.workspace.numel() < need:
-            # zeroed: the kernels expect (and leave behind) zero arrival counters
+            # zeroed: render_test's kernels expect (and leave behind) zero arrival counters
             self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
 
 
-_rt_scratch: dict = {}
-
-
-def _render_test_scratch(device, n_rays: int, min_samples: int) -> _RenderTestScratch:
+def _stream_scratch(table: dict, device) -> _StreamScratch:
     key = (device, _lib.stream_ptr(device))  # per stream: stream order is what protects the workspace
-    sc = _rt_scratch.get(key)
+    sc = table.get(key)
     if sc is None:
-        if len(_rt_scratch) >= 16:
-            _rt_scratch.clear()
-        sc = _rt_scratch[key] = _RenderTestScratch(device)
-    sc.reserve(n_rays, min_samples)
+        if len(table) >= 16:
+            table.clear()
+        sc = table[key] = _StreamScratch(device)
+    return sc
+
+
+_rt_scratch: dict = {}
+_vr_scratch: dict = {}
+
+
+def _render_test_scratch(device, n_rays: int, min_samples: int) -> _StreamScratch:
+    sc = _stream_scratch(_rt_scratch, device)
+    sc.reserve(_lib.load().nfa_render_test_workspace_bytes(n_rays, min_samples))
     return sc
 
 

@@ -432,6 +432,28 @@ int32_t nfa_searchsorted(int64_t n_query, const float* query_vals, const int64_t
                          const float* key_vals, const int64_t* key_packed_info, int64_t key_edges,
                          int64_t* ids_left, int64_t* ids_right, nfa_stream_t stream);
 
+/* replaces: the ATen composition of the proposal loss, estimators/prop_net.py:232-256 `_pdf_loss` (searchsorted, a
+ *   diff, two gathers, clip, ** 2, a division); the reference has no kernel for it.  Batched rows only: query edges /
+ *   cdfs [n_rays, q_edges], key edges / cdfs [n_rays, k_edges].  Interval j of a ray spans query edges j and j+1;
+ *   L_j = searchsorted's left id of query edge j, R_j its right id of query edge j+1 (nfa_searchsorted's search and
+ *   clipping), and loss [n_rays, q_edges-1] = clip(w - wo, min=0)^2 / (w + eps) with w = cq[j+1] - cq[j],
+ *   wo = ck[R_j] - ck[L_j], every op rounded as ATen rounds it, so the values are ATen's bit for bit.
+ *   eps: the Python scalar rounded to float.  q_edges >= 1 and k_edges >= 1; q_edges == 1 writes nothing. */
+int32_t nfa_pdf_loss_fwd(int64_t n_rays, int64_t q_edges, const float* q_vals, const float* q_cdfs, int64_t k_edges,
+                         const float* k_vals, const float* k_cdfs, float eps, float* loss, nfa_stream_t stream);
+
+/* replaces: the autograd graph of the above for the key cdfs (estimators/prop_net.py:232-256; ATen: the chain's
+ *   backwards and two gather backwards, each zeros + a float-atomic scatter_add_).  grad_loss [n_rays, q_edges-1]
+ *   (may be NULL when q_edges == 1) -> grad_k_cdfs [n_rays, k_edges], every element written (zeros included).  The
+ *   per-interval term is ATen's: where(d >= 0, -((g / (w + eps)) * (2 * c)), 0), d = w - wo, c = clip(d, min=0); key
+ *   edge k gets the sum over R_j == k in ascending j, plus the sum over L_j == k (of the negated terms) in ascending j.
+ *   No atomics: the result does not change from run to run.  q_edges - 1 > NFA_PDF_LOSS_MAX_INTERVALS is
+ *   NFA_ERR_UNSUPPORTED (a ray's ids and terms are staged in shared memory). */
+#define NFA_PDF_LOSS_MAX_INTERVALS 16384
+int32_t nfa_pdf_loss_bwd(int64_t n_rays, int64_t q_edges, const float* q_vals, const float* q_cdfs, int64_t k_edges,
+                         const float* k_vals, const float* k_cdfs, float eps, const float* grad_loss,
+                         float* grad_k_cdfs, nfa_stream_t stream);
+
 /* ----------------------------------------------------------------------- */
 /* Data-parallel exchange: sum of per-rank scalars over NVLink peer memory  */
 /* ----------------------------------------------------------------------- */

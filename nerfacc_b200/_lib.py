@@ -75,6 +75,9 @@ SIGNATURES = {
                                                                                           _c_ptr]),
     "nfa_searchsorted": (_c_i32, [_c_i64, _c_ptr, _c_ptr, _c_ptr, _c_i32, _c_i64, _c_ptr, _c_ptr, _c_i64, _c_ptr,
                                   _c_ptr, _c_ptr]),
+    "nfa_pdf_loss_fwd": (_c_i32, [_c_i64, _c_i64, _c_ptr, _c_ptr, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_ptr, _c_ptr]),
+    "nfa_pdf_loss_bwd": (_c_i32, [_c_i64, _c_i64, _c_ptr, _c_ptr, _c_i64, _c_ptr, _c_ptr, _c_f32, _c_ptr, _c_ptr,
+                                  _c_ptr]),
     "nfa_mailbox_create": (_c_i32, [_c_i32, _c_i32, _c_ptr, _c_ptr]),
     "nfa_mailbox_open": (_c_i32, [_c_ptr, _c_ptr]),
     "nfa_mailbox_close": (_c_i32, [_c_ptr]),
@@ -93,6 +96,7 @@ SIGNATURES = {
 }
 
 ABI_VERSION = 15
+PDF_LOSS_MAX_INTERVALS = 16384  # NFA_PDF_LOSS_MAX_INTERVALS: nfa_pdf_loss_bwd's longest query row, in intervals
 
 _lib = None
 launches = 0  # number of native kernel-launching calls made through this module (bench.py reports it)

@@ -5,6 +5,7 @@
 //   nerfacc/cuda/csrc/pdf.cu:168-243  compute_intervels_kernel     (second launch over the samples)
 //   nerfacc/cuda/csrc/pdf.cu:247-287  searchsorted_kernel
 //   nerfacc/cuda/csrc/pdf.cu:293-456  host wrappers (both importance_sampling overloads, searchsorted)
+//   nerfacc/estimators/prop_net.py:232-256  _pdf_loss and its autograd graph (ATen ops; no kernel in the reference)
 //
 // A ray is resampled by one warp (short rays: the proposal-network shapes) or one CTA (long rays): its
 // CDF and edge positions are staged in shared memory once, every thread inverts the CDF for its samples
@@ -317,14 +318,128 @@ __global__ void __launch_bounds__(kSearchThreads) searchsorted_kernel(SearchPara
             base = ray * p.k_edges;
             last = base + p.k_edges - 1;
         }
-        const int64_t pos = upper_bound_f<int64_t>(p.k_vals, base, last, __ldg(p.q_vals + i));
-        int64_t l = pos - 1 < last ? pos - 1 : last;
-        if (l < base) l = base;
-        int64_t r = pos < last ? pos : last;
-        if (r < base) r = base;
+        int64_t l, r;
+        search_ids<int64_t>(p.k_vals, base, last, __ldg(p.q_vals + i), l, r);
         const int64_t rel = p.q_packed ? 0 : base;  // batched queries get per-ray positions
         p.ids_left[i] = l - rel;
         p.ids_right[i] = r - rel;
+    }
+}
+
+// ---------------------------------------------------------------------------
+// Proposal loss (PropNetEstimator.compute_loss, prop_net.py `_pdf_loss`) over batched rows: query edges / cdfs
+// (n_rays, Eq), key edges / cdfs (n_rays, Ek).  Interval j of a ray spans query edges j and j+1; L_j is searchsorted's
+// left id of edge j, R_j its right id of edge j+1.  A warp per ray; key rows of up to kLossStageEdges edges are staged
+// in the warp's shared memory, longer ones are searched where they lie.
+// ---------------------------------------------------------------------------
+constexpr int kLossWarps = 8;
+constexpr int kLossCtasPerSm = 6;                             // one wave: registers allow 6 CTAs per SM
+constexpr int32_t kLossStageEdges = 512;                      // 4 KB of edges + cdfs per warp
+constexpr int64_t kLossMaxIntervals = NFA_PDF_LOSS_MAX_INTERVALS;  // the backward's per-interval rows: 12 B each
+constexpr int kLossMaxSmem = 227 * 1024;
+
+struct PdfLossParams {
+    int64_t n_rays;
+    int32_t q_edges, k_edges;
+    const float* q_vals;
+    const float* q_cdfs;
+    const float* k_vals;
+    const float* k_cdfs;
+    float eps;
+    float* loss;             // forward: (n_rays, Eq - 1)
+    const float* grad_loss;  // backward: (n_rays, Eq - 1)
+    float* grad_k_cdfs;      // backward: (n_rays, Ek)
+};
+
+// The key row of `ray`: copied into `stage` (2 * Ek floats) or read in place.
+template <bool kStage>
+NFA_D void loss_key_row(const PdfLossParams& p, int64_t ray, int lane, float* stage, const float*& kv, const float*& kc)
+{
+    kv = p.k_vals + ray * p.k_edges;
+    kc = p.k_cdfs + ray * p.k_edges;
+    if (kStage) {
+        for (int32_t i = lane; i < p.k_edges; i += 32) {
+            stage[i] = __ldg(kv + i);
+            stage[p.k_edges + i] = __ldg(kc + i);
+        }
+        __syncwarp();
+        kv = stage;
+        kc = stage + p.k_edges;
+    }
+}
+
+// L_j, R_j and w = cq[j+1] - cq[j], wo = ck[R_j] - ck[L_j] of interval j
+NFA_D void loss_interval(const PdfLossParams& p, const float* qv, const float* qc, const float* kv, const float* kc,
+                         int32_t j, int32_t& left, int32_t& right, float& w, float& wo)
+{
+    int32_t unused;
+    search_ids<int32_t>(kv, 0, p.k_edges - 1, __ldg(qv + j), left, unused);
+    search_ids<int32_t>(kv, 0, p.k_edges - 1, __ldg(qv + j + 1), unused, right);
+    w = f_sub(__ldg(qc + j + 1), __ldg(qc + j));
+    wo = f_sub(kc[right], kc[left]);
+}
+
+template <bool kStage>
+__global__ void __launch_bounds__(kLossWarps * 32, kLossCtasPerSm) pdf_loss_fwd_kernel(PdfLossParams p)
+{
+    extern __shared__ float smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* const stage = smem + (size_t)warp * 2 * p.k_edges;
+    const int32_t n = p.q_edges - 1;
+    for (int64_t ray = (int64_t)blockIdx.x * kLossWarps + warp; ray < p.n_rays;
+         ray += (int64_t)gridDim.x * kLossWarps) {
+        const float *kv, *kc;
+        loss_key_row<kStage>(p, ray, lane, stage, kv, kc);
+        const float* qv = p.q_vals + ray * p.q_edges;
+        const float* qc = p.q_cdfs + ray * p.q_edges;
+        for (int32_t j = lane; j < n; j += 32) {
+            int32_t l, r;
+            float w, wo;
+            loss_interval(p, qv, qc, kv, kc, j, l, r, w, wo);
+            p.loss[ray * n + j] = pdf_loss_term(w, wo, p.eps);
+        }
+        if (kStage) __syncwarp();  // before the next ray overwrites the stage
+    }
+}
+
+// Dense gradient of the key cdfs.  Per warp: [staged key row: 2 * Ek floats] R_j, L_j, t_j (n each).  Key edge k gets
+// (R-side sum) + (L-side sum), each summed in ascending j by pdf_loss_fold (pdf.cuh): no atomics, so the bits depend on
+// neither the launch nor the run.  Rows whose ids both do not decrease (sorted rows) search for their run; others scan
+// every j.
+template <bool kStage>
+__global__ void __launch_bounds__(kLossWarps * 32, kLossCtasPerSm) pdf_loss_bwd_kernel(PdfLossParams p,
+                                                                                       int32_t floats_per_warp)
+{
+    extern __shared__ float smem[];
+    const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* const stage = smem + (size_t)warp * floats_per_warp;
+    const int32_t n = p.q_edges - 1;
+    int32_t* const s_right = reinterpret_cast<int32_t*>(stage + (kStage ? 2 * p.k_edges : 0));
+    int32_t* const s_left = s_right + n;
+    float* const s_term = reinterpret_cast<float*>(s_left + n);
+    for (int64_t ray = (int64_t)blockIdx.x * warps + warp; ray < p.n_rays; ray += (int64_t)gridDim.x * warps) {
+        const float *kv, *kc;
+        loss_key_row<kStage>(p, ray, lane, stage, kv, kc);
+        const float* qv = p.q_vals + ray * p.q_edges;
+        const float* qc = p.q_cdfs + ray * p.q_edges;
+        for (int32_t j = lane; j < n; j += 32) {
+            int32_t l, r;
+            float w, wo;
+            loss_interval(p, qv, qc, kv, kc, j, l, r, w, wo);
+            s_right[j] = r;
+            s_left[j] = l;
+            s_term[j] = pdf_loss_grad_wo(w, wo, p.eps, __ldg(p.grad_loss + ray * n + j));
+        }
+        __syncwarp();
+        bool sorted = true;
+        for (int32_t j = lane + 1; j < n; j += 32)
+            sorted = sorted && s_right[j] >= s_right[j - 1] && s_left[j] >= s_left[j - 1];
+        sorted = __all_sync(0xffffffffu, sorted);
+        float* const gk = p.grad_k_cdfs + ray * p.k_edges;
+        for (int32_t k = lane; k < p.k_edges; k += 32)
+            gk[k] = f_add(pdf_loss_fold(s_right, s_term, n, k, sorted, false),
+                          pdf_loss_fold(s_left, s_term, n, k, sorted, true));
+        __syncwarp();  // before the next ray overwrites the rows
     }
 }
 
@@ -450,6 +565,82 @@ int32_t nfa_searchsorted(int64_t n_query, const float* query_vals, const int64_t
     const int64_t blocks = (n_query + kSearchThreads - 1) / kSearchThreads;
     const unsigned grid = (unsigned)(blocks < kNumSMs * 64 ? blocks : kNumSMs * 64);
     searchsorted_kernel<<<grid, kSearchThreads, 0, (cudaStream_t)stream>>>(p);
+    return (int32_t)cudaGetLastError();
+}
+
+static int32_t pdf_loss_params(int64_t n_rays, int64_t q_edges, const float* q_vals, const float* q_cdfs,
+                               int64_t k_edges, const float* k_vals, const float* k_cdfs, float eps, PdfLossParams& p)
+{
+    if (n_rays < 0 || q_edges < 1 || k_edges < 1 || q_edges > INT32_MAX || k_edges > INT32_MAX) return NFA_ERR_ARG;
+    p.n_rays = n_rays;
+    p.q_edges = (int32_t)q_edges;
+    p.k_edges = (int32_t)k_edges;
+    p.q_vals = q_vals;
+    p.q_cdfs = q_cdfs;
+    p.k_vals = k_vals;
+    p.k_cdfs = k_cdfs;
+    p.eps = eps;
+    p.loss = nullptr;
+    p.grad_loss = nullptr;
+    p.grad_k_cdfs = nullptr;
+    return NFA_OK;
+}
+
+int32_t nfa_pdf_loss_fwd(int64_t n_rays, int64_t q_edges, const float* q_vals, const float* q_cdfs, int64_t k_edges,
+                         const float* k_vals, const float* k_cdfs, float eps, float* loss, nfa_stream_t stream)
+{
+    PdfLossParams p;
+    const int32_t rc = pdf_loss_params(n_rays, q_edges, q_vals, q_cdfs, k_edges, k_vals, k_cdfs, eps, p);
+    if (rc != NFA_OK) return rc;
+    if (n_rays == 0 || q_edges == 1) return NFA_OK;
+    if (!q_vals || !q_cdfs || !k_vals || !k_cdfs || !loss) return NFA_ERR_ARG;
+    p.loss = loss;
+    const int64_t want = (n_rays + kLossWarps - 1) / kLossWarps;
+    const unsigned grid = (unsigned)(want < kNumSMs * kLossCtasPerSm ? want : kNumSMs * kLossCtasPerSm);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (k_edges <= kLossStageEdges)
+        pdf_loss_fwd_kernel<true><<<grid, kLossWarps * 32, (size_t)kLossWarps * 2 * k_edges * sizeof(float), s>>>(p);
+    else
+        pdf_loss_fwd_kernel<false><<<grid, kLossWarps * 32, 0, s>>>(p);
+    return (int32_t)cudaGetLastError();
+}
+
+int32_t nfa_pdf_loss_bwd(int64_t n_rays, int64_t q_edges, const float* q_vals, const float* q_cdfs, int64_t k_edges,
+                         const float* k_vals, const float* k_cdfs, float eps, const float* grad_loss,
+                         float* grad_k_cdfs, nfa_stream_t stream)
+{
+    PdfLossParams p;
+    const int32_t rc = pdf_loss_params(n_rays, q_edges, q_vals, q_cdfs, k_edges, k_vals, k_cdfs, eps, p);
+    if (rc != NFA_OK) return rc;
+    if (q_edges - 1 > kLossMaxIntervals) return NFA_ERR_UNSUPPORTED;
+    if (n_rays == 0) return NFA_OK;
+    if (!q_vals || !q_cdfs || !k_vals || !k_cdfs || !grad_k_cdfs || (q_edges > 1 && !grad_loss)) return NFA_ERR_ARG;
+    p.grad_loss = grad_loss;
+    p.grad_k_cdfs = grad_k_cdfs;
+    const bool stage = k_edges <= kLossStageEdges;
+    const int32_t floats = (int32_t)((stage ? 2 * k_edges : 0) + 3 * (q_edges - 1));
+    const size_t per_warp = (size_t)floats * sizeof(float);
+    int warps = per_warp > 0 ? (int)(kLossMaxSmem / per_warp) : kLossWarps;
+    warps = warps < kLossWarps ? warps : kLossWarps;
+    const size_t bytes = per_warp * warps;
+    // one wave: as many CTAs as fit an SM by threads and by shared memory
+    int per_sm = kLossCtasPerSm * kLossWarps / warps;
+    if (bytes > 0 && (size_t)per_sm * bytes > (size_t)kLossMaxSmem) per_sm = (int)(kLossMaxSmem / bytes);
+    const int64_t want = (n_rays + warps - 1) / warps;
+    const unsigned grid = (unsigned)(want < (int64_t)kNumSMs * per_sm ? want : (int64_t)kNumSMs * per_sm);
+    cudaStream_t s = (cudaStream_t)stream;
+#define NFA_LOSS_BWD(S)                                                                                               \
+    do {                                                                                                              \
+        if (bytes > 48 * 1024) {                                                                                      \
+            const cudaError_t e = cudaFuncSetAttribute(pdf_loss_bwd_kernel<S>,                                        \
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);      \
+            if (e != cudaSuccess) return (int32_t)e;                                                                  \
+        }                                                                                                             \
+        pdf_loss_bwd_kernel<S><<<grid, warps * 32, bytes, s>>>(p, floats);                                            \
+    } while (0)
+    if (stage) NFA_LOSS_BWD(true);
+    else NFA_LOSS_BWD(false);
+#undef NFA_LOSS_BWD
     return (int32_t)cudaGetLastError();
 }
 

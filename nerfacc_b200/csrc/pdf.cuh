@@ -1,4 +1,4 @@
-// pdf.cuh -- per-sample arithmetic of inverse-transform ("importance") sampling and searchsorted.
+// pdf.cuh -- per-sample arithmetic of inverse-transform ("importance") sampling, searchsorted and the proposal loss.
 //
 // Behaviour follows /root/reference/nerfacc/cuda/csrc/pdf.cu:22-63 (bound searches), :97-166
 // (one sample from a piecewise-linear CDF), :168-243 (edges between neighbouring samples) and the
@@ -24,6 +24,60 @@ NFA_HD Index upper_bound_f(const float* a, Index start, Index end, float v)
         else end = mid;
     }
     return start;
+}
+
+// searchsorted's pair for one query value against key edges [base, last]: key[left] <= v < key[right], both
+// clipped to the range (pdf.cu:247-287)
+template <class Index>
+NFA_HD void search_ids(const float* a, Index base, Index last, float v, Index& left, Index& right)
+{
+    const Index pos = upper_bound_f<Index>(a, base, last, v);
+    left = pos - 1 < last ? pos - 1 : last;
+    if (left < base) left = base;
+    right = pos < last ? pos : last;
+    if (right < base) right = base;
+}
+
+// Proposal loss of one query interval (estimators/prop_net.py `_pdf_loss_torch`, the reference's prop_net.py:232-256):
+// w = cq[j+1] - cq[j], wo = ck[R_j] - ck[L_j], loss = clip(w - wo, min=0) ** 2 / (w + eps), every op rounded as ATen
+// rounds it.  clip keeps a NaN (`d < 0` is false for it); `eps` is the Python scalar rounded to float, as ATen does.
+NFA_HD float pdf_loss_term(float w, float wo, float eps)
+{
+    const float d = f_sub(w, wo);
+    const float c = d < 0.f ? 0.f : d;
+    return f_div(f_mul(c, c), f_add(w, eps));
+}
+
+// d loss / d wo for the upstream gradient g, in the order ATen's autograd chain evaluates it (div, pow 2, clip, sub):
+// where(d >= 0, -((g / (w + eps)) * (2 * c)), 0).  Key edge R_j receives this, key edge L_j its negation.
+NFA_HD float pdf_loss_grad_wo(float w, float wo, float eps, float g)
+{
+    const float d = f_sub(w, wo);
+    if (!(d >= 0.f)) return 0.f;
+    return -f_mul(f_div(g, f_add(w, eps)), f_mul(2.f, d));  // c == d here
+}
+
+// Sum of the terms of the intervals j with ids[j] == k, in ascending j from +0: one key edge's share of one of the two
+// scatter_adds of ATen's gather backward.  `sorted`: ids do not decrease along j, so those intervals are the run that
+// starts at the first ids[j] >= k.
+NFA_HD float pdf_loss_fold(const int32_t* ids, const float* t, int32_t n, int32_t k, bool sorted, bool negate)
+{
+    int32_t j = 0;
+    if (sorted) {
+        int32_t hi = n;
+        while (j < hi) {
+            const int32_t mid = j + ((hi - j) >> 1);
+            if (ids[mid] < k) j = mid + 1;
+            else hi = mid;
+        }
+    }
+    float s = 0.f;
+    for (; j < n; ++j) {
+        const int32_t id = ids[j];
+        if (id == k) s = f_add(s, negate ? -t[j] : t[j]);
+        else if (sorted && id > k) break;
+    }
+    return s;
 }
 
 // number of chunk starts <= item (pdf.cu:65-80); the owning chunk is this minus one

@@ -3,7 +3,9 @@
 Same class, methods, arguments and caching protocol as /root/reference/nerfacc/estimators/prop_net.py:17-313.
 Each proposal level is one fused native launch (`nfa_importance_sampling`: sample centres, the edges
 between them and, when no gradient is needed through the edges, their s -> t mapping) plus the fused
-transmittance kernel; the reference spends two launches and ~10 ATen ops per level on the same work.
+transmittance kernel; the reference spends two launches and ~10 ATen ops per level on the same work.  The training
+loss of each level (`_pdf_loss`) is one native launch forward and one backward, with a gradient that does not change
+from run to run.
 """
 from typing import Callable, List, Optional, Tuple
 
@@ -14,10 +16,12 @@ except ImportError:  # pragma: no cover
 
 import torch
 from torch import Tensor
+from torch.autograd.function import once_differentiable
 
+from .. import _lib
 from ..data_specs import RayIntervals
 from ..pdf import _importance_sampling, searchsorted
-from ..volrend import render_transmittance_from_density
+from ..volrend import _grad_through, render_transmittance_from_density
 from .base import AbstractEstimator
 
 
@@ -167,7 +171,75 @@ def _pdf_loss(
     cdfs_key: torch.Tensor,
     eps: float = 1e-7,
 ) -> torch.Tensor:
-    """How much the query histogram exceeds the key histogram's envelope (reference prop_net.py:232-256)."""
+    """How much the query histogram exceeds the key histogram's envelope (reference prop_net.py:232-256).
+
+    Batched float32 CUDA rows with the same leading shape run ``nfa_pdf_loss_fwd`` (and ``nfa_pdf_loss_bwd`` for the
+    key cdfs' gradient): the values are :func:`_pdf_loss_torch`'s bit for bit, and the gradient is summed in a fixed
+    order, so it is the same from run to run.  Everything else -- CPU tensors, flattened queries, other dtypes, a
+    query cdf that needs a gradient (the kernels give none to the query side) -- runs :func:`_pdf_loss_torch`."""
+    q, k = segments_query.vals, segments_key.vals
+    native = (
+        q.dim() > 1 and k.dim() > 1 and q.shape[:-1] == k.shape[:-1]
+        and cdfs_query.shape == q.shape and cdfs_key.shape == k.shape
+        and q.shape[-1] >= 1 and k.shape[-1] >= 1 and q.shape[-1] - 1 <= _lib.PDF_LOSS_MAX_INTERVALS
+        and all(t.is_cuda and t.dtype == torch.float32 for t in (q, cdfs_query, k, cdfs_key))
+        and not _grad_through(cdfs_query)
+    )
+    if not native:
+        return _pdf_loss_torch(segments_query, cdfs_query, segments_key, cdfs_key, eps)
+    if _grad_through(cdfs_key):
+        return _PdfLoss.apply(q, cdfs_query, k, cdfs_key, eps)
+    return _pdf_loss_fwd(q, cdfs_query, k, cdfs_key, eps)
+
+
+def _loss_rows(q: Tensor, cq: Tensor, k: Tensor, ck: Tensor):
+    """(R, Eq) and (R, Ek) contiguous rows of the batched operands."""
+    eq, ek = q.shape[-1], k.shape[-1]
+    return (q.reshape(-1, eq).contiguous(), cq.reshape(-1, eq).contiguous(), k.reshape(-1, ek).contiguous(),
+            ck.reshape(-1, ek).contiguous())
+
+
+def _pdf_loss_fwd(q: Tensor, cq: Tensor, k: Tensor, ck: Tensor, eps: float) -> Tensor:
+    rq, rcq, rk, rck = _loss_rows(q, cq, k, ck)
+    n_rays, eq, ek = rq.shape[0], rq.shape[1], rk.shape[1]
+    loss = torch.empty(q.shape[:-1] + (eq - 1,), dtype=torch.float32, device=q.device)
+    if loss.numel() > 0:
+        _lib.call("nfa_pdf_loss_fwd", q.device, n_rays, eq, rq.data_ptr(), rcq.data_ptr(), ek, rk.data_ptr(),
+                  rck.data_ptr(), eps, loss.data_ptr())
+    return loss
+
+
+class _PdfLoss(torch.autograd.Function):
+    """Per-interval proposal loss; the gradient flows to the key cdfs only (``_pdf_loss`` routes the other cases)."""
+
+    @staticmethod
+    def forward(ctx, q: Tensor, cq: Tensor, k: Tensor, ck: Tensor, eps: float):
+        ctx.save_for_backward(q, cq, k, ck)
+        ctx.eps = eps
+        return _pdf_loss_fwd(q, cq, k, ck, eps)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad: Tensor):
+        q, cq, k, ck = ctx.saved_tensors
+        rq, rcq, rk, rck = _loss_rows(q, cq, k, ck)
+        n_rays, eq, ek = rq.shape[0], rq.shape[1], rk.shape[1]
+        grad_ck = torch.empty(ck.shape, dtype=torch.float32, device=ck.device)
+        if n_rays > 0:
+            g = grad.reshape(n_rays, eq - 1).contiguous()
+            _lib.call("nfa_pdf_loss_bwd", q.device, n_rays, eq, rq.data_ptr(), rcq.data_ptr(), ek, rk.data_ptr(),
+                      rck.data_ptr(), ctx.eps, _lib.ptr(g) if g.numel() > 0 else None, grad_ck.data_ptr())
+        return None, None, None, grad_ck, None
+
+
+def _pdf_loss_torch(
+    segments_query: RayIntervals,
+    cdfs_query: torch.Tensor,
+    segments_key: RayIntervals,
+    cdfs_key: torch.Tensor,
+    eps: float = 1e-7,
+) -> torch.Tensor:
+    """``_pdf_loss`` as ATen ops, the reference's formulation (prop_net.py:232-256)."""
     ids_left, ids_right = searchsorted(segments_key, segments_query)
     if segments_query.vals.dim() > 1:
         w = cdfs_query[..., 1:] - cdfs_query[..., :-1]

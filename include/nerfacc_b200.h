@@ -73,7 +73,8 @@ int32_t nfa_occ_pack(int32_t n_grids, int32_t rx, int32_t ry, int32_t rz, const 
 
 /* Grid maintenance (OccGridEstimator._update, nerfacc/estimators/occ_grid.py:367-404).
  * nfa_occ_ema_update: occs[cell_ids[i]] = max(occs[cell_ids[i]] * ema_decay, occ[i]) (:395-398); a cell named more
- *   than once gets the largest of its results.  scratch: n floats.
+ *   than once gets the largest of its results in the order -inf < ... < -0.0 < +0.0 < ... < +inf, NaN if any
+ *   result is NaN.  scratch: n floats.
  * nfa_occ_threshold_pack: thre = min(mean(occs[occs >= 0]), occ_thre) (:400-402), binaries = occs > thre (:403-404)
  *   written as bool bytes AND as the derived cache nfa_occ_pack would build from them (words / coarse / bounds),
  *   one pass, no host synchronisation.  workspace: nfa_occ_threshold_workspace_bytes(n_cells) bytes, 16-byte

@@ -42,16 +42,18 @@ __global__ void __launch_bounds__(kUpdThreads) occ_ema_gather_kernel(int64_t n, 
         fresh[i] = max_nan(__fmul_rn(occs[ids[i]], decay), occ[i]);
 }
 
-// float max through integer atomics: non-negative floats order like signed ints, negative ones like reversed
-// unsigned ints.  A NaN is stored as is (and stays: the integer compare below never replaces it by a number
-// that is not also the result of some draw).
+// float max through integer atomics: floats with a clear sign bit order like signed ints, those with the sign bit
+// set like reversed unsigned ints.  The path is chosen by the sign bit, not by `v >= 0`: -0.0 compares equal to
+// +0.0 but its bits are INT_MIN, which the signed max would never prefer to the -INFINITY the reset left.  So the
+// draws reduce in the total order -inf < ... < -0.0 < +0.0 < ... < +inf.  A NaN is stored as is (and stays: the
+// integer compare below never replaces it by a number that is not also the result of some draw).
 __device__ __forceinline__ void atomic_max_float(float* addr, float v)
 {
     if (v != v) {
         *addr = v;
         return;
     }
-    if (v >= 0.0f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+    if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 

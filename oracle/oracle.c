@@ -712,7 +712,8 @@ ORC_API void orc_searchsorted(
 /* occ_grid.py:395-398  occs[ids] = maximum(occs[ids] * ema_decay, occ).  The right-hand side is evaluated on the
  * OLD values for every draw before anything is written (index_put_); when `ids` names a cell more than once
  * torch keeps one of the candidates (the last one on the CPU, an arbitrary one on CUDA) -- this restatement
- * keeps the largest, the only rule that does not depend on the order of the writes.  `fresh`: n floats. */
+ * keeps the largest, the only rule that does not depend on the order of the writes: largest in the total order
+ * -inf < ... < -0.0 < +0.0 < ... < +inf, NaN if any candidate is NaN.  `fresh`: n floats. */
 ORC_API void orc_occ_ema_update(int64_t n, const int64_t* ids, const float* occ, float ema_decay, float* occs,
                                 float* fresh)
 {
@@ -724,7 +725,7 @@ ORC_API void orc_occ_ema_update(int64_t n, const int64_t* ids, const float* occ,
     for (int64_t i = 0; i < n; ++i) {
         float* dst = occs + ids[i];
         if (fresh[i] != fresh[i] || *dst != *dst) *dst = NAN;
-        else if (fresh[i] > *dst) *dst = fresh[i];
+        else if (fresh[i] > *dst || (fresh[i] == *dst && signbit(*dst) && !signbit(fresh[i]))) *dst = fresh[i];
     }
 }
 

@@ -35,3 +35,17 @@ def test_oracle_update_matches_reference(orc, case):
     assert thre <= occ_thre
     np.testing.assert_array_equal(bins.reshape(want_bin.shape), want_bin)
     assert (~bins[want < 0]).all()                                  # invisible cells stay empty
+
+
+def test_oracle_update_keeps_the_largest_in_the_total_order(orc):
+    """A cell drawn more than once keeps its largest result in the order -0.0 < +0.0, whichever draw comes first, a
+    -0.0 result is not lost to the -inf a drawn cell starts from, and NaN wins."""
+    draws = [(0.0, -0.0), (-0.0, 0.0), (-0.0,), (-0.0, -0.5), (-0.5, -0.0), (np.nan, 1.0), (1.0, np.nan)]
+    ids = np.array([c for c, d in enumerate(draws) for _ in d], np.int64)
+    occ = np.array([v for d in draws for v in d], np.float32)
+    before = np.full(len(draws), -np.inf, np.float32)  # -inf * 1.0 = -inf: every result is the draw itself
+    got = orc.occ_ema_update(before, ids, occ, 1.0)
+    want = np.array([0.0, 0.0, -0.0, -0.0, -0.0, np.nan, np.nan], np.float32)
+    np.testing.assert_array_equal(np.isnan(got), np.isnan(want))
+    ok = ~np.isnan(want)
+    np.testing.assert_array_equal(got[ok].view(np.uint32), want[ok].view(np.uint32))
